@@ -96,15 +96,28 @@ __device__ __forceinline__ void cp_async_wait() {
   asm volatile("cp.async.wait_group %0;\n" ::"n"(N));
 }
 
-// Native f64 tensor-core op: lowers to one DMMA instruction.
-// Fragment layout (PTX ISA, mma.m8n8k4 f64): g = lane>>2, t = lane&3:
-//   a  = A[g][t]          (8x4, row)
-//   b  = B[t][g]          (4x8, col)
-//   c0 = C[g][2t], c1 = C[g][2t+1]
-__device__ __forceinline__ void dmma884(double& c0, double& c1, double a, double b) {
-  asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n"
-               : "+d"(c0), "+d"(c1)
-               : "d"(a), "d"(b));
+// The widest f64 tensor-core op of sm_90: one SASS DMMA.16x8x16, 8x the work of the m8n8k4 shape per instruction
+// (which cannot keep the H100's f64 tensor pipe full, profiles/r03_f64_peaks.log).
+// Fragment layout (PTX ISA, mma.m16n8k16 f64): g = lane>>2, t = lane&3:
+//   a[v] = A[g + 8 (v & 1)][t + 4 (v >> 1)]   (16x16, row), v = 0..7
+//   b[i] = B[t + 4 i][g]                      (16x8, col),  i = 0..3
+//   c0 = C[g][2t], c1 = C[g][2t+1], c2 = C[g+8][2t], c3 = C[g+8][2t+1]
+// Any bijection of the 16 k indices is allowed as long as A and B use the same one (the product is a sum over k).
+__device__ __forceinline__ void dmma16816(double& c0, double& c1, double& c2, double& c3, const double (&a)[8],
+                                          const double (&b)[4]) {
+  asm volatile(
+      "mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7,%8,%9,%10,%11}, {%12,%13,%14,%15}, "
+      "{%0,%1,%2,%3};\n"
+      : "+d"(c0), "+d"(c1), "+d"(c2), "+d"(c3)
+      : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(a[4]), "d"(a[5]), "d"(a[6]), "d"(a[7]), "d"(b[0]), "d"(b[1]),
+        "d"(b[2]), "d"(b[3]));
+}
+// The same layout truncated to k = 8 (a[0..3], b[0..1]; one SASS DMMA.16x8x8): half the fragment registers per instruction.
+__device__ __forceinline__ void dmma1688(double& c0, double& c1, double& c2, double& c3, const double (&a)[4],
+                                         const double (&b)[2]) {
+  asm volatile("mma.sync.aligned.m16n8k8.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
+               : "+d"(c0), "+d"(c1), "+d"(c2), "+d"(c3)
+               : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(b[0]), "d"(b[1]));
 }
 #endif  // __CUDACC__
 

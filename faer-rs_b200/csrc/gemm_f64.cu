@@ -1,10 +1,9 @@
 // f64 GEMM / structured GEMM kernel, see gemm_f64.cuh for the reference semantics it implements.
 //
 // Design (H100, sm_90a):
-//   * math: mma.sync.m8n8k4.f64 -> DMMA (the f64 tensor op; wgmma has no f64 type).
-//     The H100 data sheet (67 TFLOP/s FP64 tensor, 132 SMs) works out to ~128 f64 FMA/clk/SM => a 128x128x16 CTA
-//     k-step is ~2048 clk of tensor work; one __syncthreads per k-step and a 4-stage cp.async ring were sized for half
-//     that rate and have not been re-tuned for the H100 (DESIGN.md §7).
+//   * math: mma.sync.m16n8k16.f64 -> one DMMA.16x8x16 per 16 x 8 block and 16-deep k-step (wgmma has no f64 type).
+//     The m8n8k4 shape sustains only half of the H100's f64 tensor rate; the wide shapes reach ~128 f64 FMA/clk/SM
+//     (profiles/r03_f64_peaks.log).
 //   * operands staged with cp.async (16 B vectors when the view is aligned, 8 B otherwise => any stride,
 //     any sign) into padded shared tiles; pad of 4 doubles makes every fragment load (8 rows x 4 k of
 //     8-byte words per half-warp) hit 16 distinct 8-byte banks.
@@ -143,6 +142,7 @@ __global__ void __launch_bounds__(Cfg::THREADS) gemm_f64_kernel(const GemmF64Par
   constexpr int BM = Cfg::BM, BN = Cfg::BN, BK = Cfg::BK, STAGES = Cfg::STAGES, THREADS = Cfg::THREADS;
   constexpr int WMI = Cfg::WMI, WNI = Cfg::WNI;
   constexpr bool SWZ = Cfg::SWZ;
+  static_assert(BK == 16 && WMI % 2 == 0, "the main loop issues 16 x 8 x 16 DMMAs");
   using TA = OpTile<BM, BK, AK, SWZ>;
   using TB = OpTile<BN, BK, !BNM, SWZ>;  // rhs: K-major when b_rs == 1
   extern __shared__ __align__(16) double smem[];
@@ -229,18 +229,21 @@ __global__ void __launch_bounds__(Cfg::THREADS) gemm_f64_kernel(const GemmF64Par
       if (nk < nkt) load_stage(nk % STAGES, nk);
       cp_async_commit();
     }
+    // one 16-deep DMMA per 16 x 8 block (rows 8 (2 ip) .. 8 (2 ip + 2) of the warp tile x 8 columns), k = t + 4 q
+    double a[WMI / 2][8], b[WNI][4];
 #pragma unroll
-    for (int kk = 0; kk < BK; kk += 4) {
-      double a[WMI], b[WNI];
+    for (int ip = 0; ip < WMI / 2; ++ip)
 #pragma unroll
-      for (int i = 0; i < WMI; ++i) a[i] = a_s[TA::idx(wm0 + i * 8 + g, kk + t)];
+      for (int v = 0; v < 8; ++v) a[ip][v] = a_s[TA::idx(wm0 + (2 * ip + (v & 1)) * 8 + g, 4 * (v >> 1) + t)];
 #pragma unroll
-      for (int j = 0; j < WNI; ++j) b[j] = b_s[TB::idx(wn0 + j * 8 + g, kk + t)];
+    for (int j = 0; j < WNI; ++j)
 #pragma unroll
-      for (int i = 0; i < WMI; ++i)
+      for (int q = 0; q < 4; ++q) b[j][q] = b_s[TB::idx(wn0 + j * 8 + g, 4 * q + t)];
 #pragma unroll
-        for (int j = 0; j < WNI; ++j) dmma884(acc[i][j][0], acc[i][j][1], a[i], b[j]);
-    }
+    for (int ip = 0; ip < WMI / 2; ++ip)
+#pragma unroll
+      for (int j = 0; j < WNI; ++j)
+        dmma16816(acc[2 * ip][j][0], acc[2 * ip][j][1], acc[2 * ip + 1][j][0], acc[2 * ip + 1][j][1], a[ip], b[j]);
   }
   cp_async_wait<0>();
 
@@ -291,7 +294,8 @@ __global__ void __launch_bounds__(Cfg::THREADS) gemm_f64_kernel(const GemmF64Par
 using CfgL = TileCfg<2, 4, 8, 4, 16, 4>;   // 128 x 128 x 16, 256 threads, warp tile 64 x 32
 using CfgS = TileCfg<2, 2, 4, 4, 16, 4>;   // 64 x 64 x 16, 128 threads, warp tile 32 x 32
 using CfgS3 = TileCfg<2, 2, 4, 4, 16, 3>;  // 64 x 64 x 16, 3 stages (57 KB => 3 CTAs/SM)
-using CfgZ4 = TileCfg<2, 2, 4, 4, 16, 4, true>;  // 64 x 64 x 16 swizzled, 4 stages (64 KB => 3 CTAs/SM)
+using CfgZ4 = TileCfg<2, 2, 4, 4, 16, 4, true>;  // 64 x 64 x 16 swizzled, 4 stages (64 KB; 3 CTAs/SM by shared memory,
+                                                 // 2 in the layout variants that need more than 168 registers)
 
 // development knob: FAER_B200_GEMM_CFG=1..10 forces one tile configuration (0/unset = heuristic)
 inline int forced_cfg() {
@@ -485,12 +489,13 @@ void gemm_f64(cudaStream_t stream, VD dst, int dst_struct, int accum, VCD lhs, i
   // large rectangular-operand products: the TMA-fed warp-specialised kernel (gemm_f64_ws.cuh)
   if (ws_mode() != 0 && !split_ws) {
     // Heuristic: the ws kernel takes products whose 128 x 64 tiles fill >= 3 waves of two CTAs per SM and whose
-    // contraction is deep enough to amortise a tile's epilogue; the cp.async kernel (64 x 64 tiles, three CTAs per SM)
-    // keeps short contractions into a triangular destination and products with few tiles.
+    // contraction is deep enough to amortise a tile's epilogue (k >= 512: at k = 256 the cp.async kernel is faster even on
+    // a full 16384 x 16384 update, profiles/r03_gemm_f64_shapes.log); the cp.async kernel (64 x 64 tiles, three CTAs per
+    // SM) keeps short contractions and products with few tiles.
     long long tiles_ws = (long long)((p.m + ws64::BM - 1) / ws64::BM) * ((p.n + ws64::BN - 1) / ws64::BN);
     if (dst_struct != RECT) tiles_ws = tiles_ws / 2 + 1;
     const long long wave = 2ll * stream_sms(stream);
-    const bool deep = dst_struct == RECT ? p.k >= 256 : p.k >= 512;
+    const bool deep = p.k >= 512;
     if (ws_mode() == 2 || (tiles_ws >= 3 * wave && deep)) {
       if (prof) profile_record_start(stream);
       const bool took = ws64::try_gemm_f64_ws(stream, p);

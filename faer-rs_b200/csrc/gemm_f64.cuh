@@ -1,4 +1,4 @@
-// G1/G2: f64 GEMM on the native f64 tensor path (DMMA.8x8x4 via mma.sync.m8n8k4.f64).
+// G1/G2: f64 GEMM on the native f64 tensor path (DMMA.16x8x16 / DMMA.16x8x8 via mma.sync.m16n8k16 / m16n8k8 .f64).
 //
 // Computes   dst(struct) = [dst +] alpha * lhs(struct) * rhs(struct)
 // with faer's semantics:

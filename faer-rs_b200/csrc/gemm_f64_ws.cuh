@@ -5,8 +5,10 @@
 // updates of LLT (SYRK), LU and QR and `matmul` itself. Structured INPUTS, odd strides and tiny / tall-skinny problems
 // stay on the cp.async kernel (gemm_f64.cu).
 //
-// wgmma has no f64 type; the f64 tensor op of sm_90a is the warp-level mma.sync.m8n8k4 (SASS DMMA). So "tensor-core
-// tiles fed by TMA" means here:
+// wgmma has no f64 type; the f64 tensor ops of sm_90a are the warp-level mma.sync shapes m8n8k4, m16n8k4, m16n8k8 and
+// m16n8k16 (SASS DMMA). Only the 16-row shapes reach the full f64 tensor rate (profiles/r03_f64_peaks.log); this kernel
+// issues m16n8k8 (the 16-deep shape's fragments do not fit beside 128 accumulator registers). So "tensor-core tiles fed by
+// TMA" means here:
 //   * CTAs of bounded persistence (each owns `tiles_per_cta` consecutive tiles, sized so that a CTA lives ~100 us: long
 //     enough to amortise its start-up and to overlap every epilogue with the next tile's loads, short enough that the SMs
 //     turn over and a higher-priority stream — the panel chain of the look-ahead factorizations — gets in), 2 per SM,
@@ -16,8 +18,8 @@
 //   * producer: one elected lane issues cp.async.bulk.tensor (TMA, SASS UTMALDG) loads of both operand slabs into a
 //     4-stage ring of 128B-swizzled shared-memory tiles and signals `full[s]` through the mbarrier's transaction count;
 //     out-of-range rows / columns / k are zero-filled by the TMA unit (no predication in the loop);
-//   * consumers: wait `full[s]`, read DMMA fragments with conflict-free 8-byte loads (see "k permutation"), issue 128
-//     DMMAs per stage, then one lane per warp arrives on `empty[s]`. There is no CTA-wide barrier in the main loop; the
+//   * consumers: wait `full[s]`, read DMMA fragments with conflict-free 8-byte loads (see "k permutation"), issue 32
+//     DMMA.16x8x8 per stage, then one lane per warp arrives on `empty[s]`. There is no CTA-wide barrier in the main loop; the
 //     producer runs up to 4 stages ahead, ACROSS tile boundaries, so the next tile's operands land while the epilogue
 //     of the current one runs, and the second CTA of the SM keeps the DMMA pipe busy during that epilogue;
 //   * epilogue: registers -> global directly (alpha, optional accumulate with the 16 old values of a row block loaded
@@ -26,11 +28,13 @@
 // Shared-memory layouts (both produced by TMA with CU_TENSOR_MAP_SWIZZLE_128B, rows of 128 B):
 //   MN-major operand (unit stride along m or n; e.g. column-major lhs): boxes of 16 (mn) x 16 (k): [blk][k][16 mn]
 //   K-major  operand (unit stride along k; e.g. column-major rhs):      one box 16 (k) x rows:     [mn][16 k]
-// k permutation: a DMMA contracts 4 k-indices, lane t = lane & 3 supplying index K4(s, t) for both operands. Any
-// partition of the 16 k-indices of a stage into 4 such sets is valid (a sum is a sum); {0,3,12,15} ^ {0,1,4,5} makes
+// k permutation: lane t = lane & 3 supplies, in fragment k slot q (k = t + 4q of the PTX layout), stage index K4(q, t)
+// for both operands. Any bijection of the 16 k-indices of a stage is valid (a sum is a sum); {0,3,12,15} ^ {0,1,4,5} makes
 // the 16 eight-byte fragment loads of a half-warp hit 16 distinct banks in BOTH layouts under the 128B swizzle.
 #pragma once
 #include <cuda.h>
+
+#include <algorithm>
 
 #include "gemm_f64.cuh"
 #include "runtime.cuh"
@@ -218,8 +222,8 @@ gemm_f64_ws_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
   if constexpr (VAR != 1) asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
   const int g = lane >> 2, t = lane & 3;
   const int wm0 = (warp - 4) * (WMI * 8);  // warp tile rows [wm0, wm0 + 32) x all 64 columns
-  // per-lane fragment offsets for the 4 DMMA sub-steps of a stage: k index K4(s, t) = {0,3,12,15}[t] ^ {0,1,4,5}[s]
-  uint32_t offA[4][2], offB[4][2];  // [sub-step][parity of the 8-row block] (MN-major) / [sub-step][0] (K-major)
+  // per-lane fragment offsets for the 4 k slots of a stage: k index K4(q, t) = {0,3,12,15}[t] ^ {0,1,4,5}[q]
+  uint32_t offA[4][2], offB[4][2];  // [k slot][parity of the 8-row block] (MN-major) / [k slot][0] (K-major)
   {
     const int base_k = (t == 0) ? 0 : (t == 1) ? 3 : (t == 2) ? 12 : 15;
 #pragma unroll
@@ -280,24 +284,34 @@ gemm_f64_ws_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
       }
       mbar_wait(&full[s], ph);
       const uint32_t sa = smem_base + s * STAGE_BYTES, sb = sa + A_BYTES;
+      // two DMMA.16x8x8 per 16 x 8 block and stage (the 16-deep shape's fragments do not fit beside the 128 accumulator
+      // registers): half h contracts fragment k slots q = 2h + (v >> 1) (A) / 2h + i (B), i.e. stage indices K4(q, t).
+      // A fragments of the whole warp tile, B fragments one 8-column block at a time.
 #pragma unroll
-      for (int ss = 0; ss < 4; ++ss) {
-        double a[WMI], b[WNI];
+      for (int h = 0; h < 2; ++h) {
+        double a[WMI / 2][4];
 #pragma unroll
-        for (int i = 0; i < WMI; ++i) {
-          if constexpr (A_KMAJOR) a[i] = lds64(sa + offA[ss][0] + i * 8 * 128);
-          else a[i] = lds64(sa + offA[ss][i & 1] + (i >> 1) * 2048);
-          if constexpr (SPICY) a[i] *= dk[ss];
-        }
+        for (int ip = 0; ip < WMI / 2; ++ip)
+#pragma unroll
+          for (int v = 0; v < 4; ++v) {
+            const int i = 2 * ip + (v & 1), q = 2 * h + (v >> 1);
+            if constexpr (A_KMAJOR) a[ip][v] = lds64(sa + offA[q][0] + i * 8 * 128);
+            else a[ip][v] = lds64(sa + offA[q][i & 1] + (i >> 1) * 2048);
+            if constexpr (SPICY) a[ip][v] *= dk[q];
+          }
 #pragma unroll
         for (int j = 0; j < WNI; ++j) {
-          if constexpr (B_KMAJOR) b[j] = lds64(sb + offB[ss][0] + j * 8 * 128);
-          else b[j] = lds64(sb + offB[ss][j & 1] + (j >> 1) * 2048);
+          double b[2];
+#pragma unroll
+          for (int v = 0; v < 2; ++v) {
+            const int q = 2 * h + v;
+            if constexpr (B_KMAJOR) b[v] = lds64(sb + offB[q][0] + j * 8 * 128);
+            else b[v] = lds64(sb + offB[q][j & 1] + (j >> 1) * 2048);
+          }
+#pragma unroll
+          for (int ip = 0; ip < WMI / 2; ++ip)
+            dmma1688(acc[2 * ip][j][0], acc[2 * ip][j][1], acc[2 * ip + 1][j][0], acc[2 * ip + 1][j][1], a[ip], b);
         }
-#pragma unroll
-        for (int i = 0; i < WMI; ++i)
-#pragma unroll
-          for (int j = 0; j < WNI; ++j) dmma884(acc[i][j][0], acc[i][j][1], a[i], b[j]);
       }
       if constexpr (VAR != 5) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
       __syncwarp();
@@ -435,8 +449,11 @@ inline bool try_gemm_f64_ws(cudaStream_t stream, const GemmF64Params& q, const S
   const bool okA = ak ? make_map(&mapA, q.A, q.k, q.m, q.a_rs, BM) : make_map(&mapA, q.A, q.m, q.k, q.a_cs, 16);
   const bool okB = bk ? make_map(&mapB, q.B, q.k, q.n, q.b_cs, BN) : make_map(&mapB, q.B, q.n, q.k, q.b_rs, 16);
   if (!okA || !okB) return false;
-  // tiles per CTA shrink with k so that a CTA stays short-lived (on the order of 100 us)
-  p.tiles_per_cta = (int)std::max<long long>(1, std::min<long long>(8, 768 / std::max(q.k, 1)));
+  // tiles per CTA shrink with k so that a CTA stays short-lived (on the order of 50 us at 128 f64 FMA / clock / SM), and
+  // never below two CTAs per SM while the tiles allow it (fewer would leave SMs idle in small launches)
+  p.sm_slots = stream_sms(stream);
+  const long long tpc_fill = std::max<long long>(1, (tiles + 2ll * p.sm_slots - 1) / (2ll * p.sm_slots));
+  p.tiles_per_cta = (int)std::max<long long>(1, std::min<long long>({8, 768 / std::max(q.k, 1), tpc_fill}));
   const int grid = (int)((tiles + p.tiles_per_cta - 1) / p.tiles_per_cta);
   {
     static int stagger = -1;
@@ -444,9 +461,8 @@ inline bool try_gemm_f64_ws(cudaStream_t stream, const GemmF64Params& q, const S
       const char* e = getenv("FAER_B200_WS_STAGGER");  // 0 switches the stagger off (dev knob)
       stagger = e ? atoi(e) : 1;
     }
-    p.sm_slots = stream_sms(stream);
-    // half a tile at the full rate of one SM: (k / 16) k-steps x 512 DMMA x 4 clocks / 2
-    p.stagger_cycles = (stagger && grid >= 2 * p.sm_slots) ? (long long)((q.k + BK - 1) / BK) * 1024 : 0;
+    // half a tile at the full rate of one SM: (k / 16) k-steps x 128 x 64 x 16 FMA / (128 FMA / clock) / 2
+    p.stagger_cycles = (stagger && grid >= 2 * p.sm_slots) ? (long long)((q.k + BK - 1) / BK) * 512 : 0;
   }
   // one opt-in to > 48 KB of dynamic shared memory per kernel variant
   static bool configured[16] = {};

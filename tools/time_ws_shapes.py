@@ -23,7 +23,8 @@ def best(f, reps=5):
 
 
 tag = f"stagger={os.environ.get('FAER_B200_WS_STAGGER', '1')}"
-for (n, k) in [(16128, 256), (16128, 512), (8192, 256), (4096, 256)]:
+# lower-triangular updates of the headline LLT (k = 256, and k = 128 in its last 6144 columns), and deeper ones
+for (n, k) in [(16128, 256), (12288, 256), (8192, 256), (4096, 256), (1024, 256), (6016, 128), (3072, 128), (16128, 512)]:
     P = torch.randn((k, n), dtype=torch.float64, device=dev).T
     Cm = torch.randn((n, n), dtype=torch.float64, device=dev).T
     line = f"{tag} SYRK(lower) n={n} k={k}:"
@@ -33,7 +34,9 @@ for (n, k) in [(16128, 256), (16128, 512), (8192, 256), (4096, 256)]:
         line += f"  mode {mode}: {ms:.3f} ms {n * n * k / ms / 1e9:.2f} TF"
     print(line, flush=True)
     del P, Cm
-for (m, n, k) in [(16384, 16384, 256), (16384, 16384, 512), (8192, 8192, 512), (16384, 512, 512), (16384, 256, 256)]:
+# rectangular: LU / GEMM updates, and the LLT panel chain's rows x 256 x 256 updates
+for (m, n, k) in [(16384, 16384, 256), (16384, 16384, 512), (8192, 8192, 512), (16384, 512, 512), (16128, 256, 256),
+                  (8192, 256, 256), (2048, 256, 256)]:
     L = torch.randn((k, m), dtype=torch.float64, device=dev).T
     U = torch.randn((n, k), dtype=torch.float64, device=dev).T
     Cm = torch.randn((n, m), dtype=torch.float64, device=dev).T
