@@ -488,17 +488,22 @@ void gemm_f64(cudaStream_t stream, VD dst, int dst_struct, int accum, VCD lhs, i
   }
   // large rectangular-operand products: the TMA-fed warp-specialised kernel (gemm_f64_ws.cuh)
   if (ws_mode() != 0 && !split_ws) {
-    // Heuristic: the ws kernel takes products whose 128 x 64 tiles fill >= 3 waves of two CTAs per SM and whose
-    // contraction is deep enough to amortise a tile's epilogue (k >= 512: at k = 256 the cp.async kernel is faster even on
-    // a full 16384 x 16384 update, profiles/r03_gemm_f64_shapes.log); the cp.async kernel (64 x 64 tiles, three CTAs per
-    // SM) keeps short contractions and products with few tiles.
-    long long tiles_ws = (long long)((p.m + ws64::BM - 1) / ws64::BM) * ((p.n + ws64::BN - 1) / ws64::BN);
-    if (dst_struct != RECT) tiles_ws = tiles_ws / 2 + 1;
-    const long long wave = 2ll * stream_sms(stream);
-    const bool deep = p.k >= 512;
-    if (ws_mode() == 2 || (tiles_ws >= 3 * wave && deep)) {
+    // Heuristic. Triangular destinations with k <= 512 and >= 3 waves of 128 x 128 tiles (one CTA per SM) take the wide
+    // configuration: the SYRK trailing updates of LLT. Other products take the narrow one when their 128 x 64 tiles fill
+    // >= 3 waves of two CTAs per SM and their contraction is deep enough to amortise a tile's epilogue (k >= 512: at
+    // k = 256 the cp.async kernel is faster even on a full 16384 x 16384 update, profiles/r03_gemm_f64_shapes.log); the
+    // cp.async kernel (64 x 64 tiles, three CTAs per SM) keeps short contractions and products with few tiles.
+    // gemm_ws = 2 forces the narrow configuration, 3 the wide one.
+    const int sms = stream_sms(stream);
+    const bool wide = ws_mode() == 3 ||
+                      (ws_mode() == 1 && dst_struct != RECT && p.k <= 512 &&
+                       ws64::ws_tiles(p.m, p.n, dst_struct, ws64::Shape<true>::BN) >= 3ll * sms);
+    long long tiles_narrow = (long long)((p.m + ws64::BM - 1) / ws64::BM) * ((p.n + ws64::Shape<false>::BN - 1) / ws64::Shape<false>::BN);
+    if (dst_struct != RECT) tiles_narrow = tiles_narrow / 2 + 1;
+    const bool narrow = ws_mode() == 2 || (ws_mode() == 1 && tiles_narrow >= 3 * 2ll * sms && p.k >= 512);
+    if (wide || narrow) {
       if (prof) profile_record_start(stream);
-      const bool took = ws64::try_gemm_f64_ws(stream, p);
+      const bool took = ws64::try_gemm_f64_ws(stream, p, nullptr, wide);
       if (took) {
         if (prof) profile_record_stop(stream, flops);
         return;
@@ -577,7 +582,7 @@ void spicy_matmul_f64(cudaStream_t st, VD C, int c_struct, const long long* row_
     p.B = B.ptr; p.b_rs = B.rs; p.b_cs = B.cs; p.b_struct = RECT;
     p.C = C.ptr; p.c_rs = C.rs; p.c_cs = C.cs; p.c_struct = c_struct;
     p.alpha = alpha; p.accum = accum; p.k_split_len = 0; p.c_split_stride = 0;
-    const long long tiles = (long long)((m + ws64::BM - 1) / ws64::BM) * ((n + ws64::BN - 1) / ws64::BN);
+    const long long tiles = (long long)((m + ws64::BM - 1) / ws64::BM) * ((n + ws64::Shape<false>::BN - 1) / ws64::Shape<false>::BN);
     if (ws_mode() == 2 || (tiles >= 32 && k >= 16)) {
       ws64::Spicy sp;
       sp.row_idx = row_idx; sp.col_idx = col_idx; sp.diag = diag; sp.diag_stride = diag_stride;

@@ -42,12 +42,35 @@
 namespace fb {
 namespace ws64 {
 
-constexpr int BM = 128, BN = 64, BK = 16, STAGES = 4;
-constexpr int CONSUMERS = 4;                       // consumer warps (warpgroup 1), stacked along m: warp tile 32 x 64
-constexpr int THREADS = 256;                       // warpgroup 0: producer (warp 0 works), warpgroup 1: consumers
-constexpr int WMI = 4, WNI = 8;                    // 8 x 8 DMMA blocks per warp tile
-constexpr int A_BYTES = BM * BK * 8, B_BYTES = BN * BK * 8, STAGE_BYTES = A_BYTES + B_BYTES;  // 16 KB + 8 KB
-constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*alignment*/ + 128 /*barriers*/;
+constexpr int BM = 128, BK = 16;
+constexpr int WMI = 4, WNI = 8;                    // 8 x 8 DMMA blocks per warp tile (32 x 64)
+constexpr int A_BYTES = BM * BK * 8;               // 16 KB
+
+// Two configurations of the same kernel.
+//   narrow (WIDE = false): CTA tile 128 x 64, 4 consumer warps stacked along m, 4 stages of 24 KB, two CTAs per SM, the
+//     register epilogue for every tile.
+//   wide (WIDE = true): CTA tile 128 x 128, 8 consumer warps (4 along m x 2 along n, two consumer warpgroups), 3 stages of
+//     32 KB and a 128 KB destination buffer, one CTA per SM. Per DMMA it reads half the operand bytes of the 64 x 64
+//     cp.async tile (16 instead of 32 B per clock and SM at the full DMMA rate). Tiles that lie wholly inside the kept
+//     part of dst are combined in shared memory: the producer TMA-loads the old dst tile while the tile's main loop runs
+//     (Add mode), the consumers write alpha * acc [+ old] into the buffer and one thread TMA-stores it, so the next tile's
+//     main loop starts while the store drains. Tiles that straddle the diagonal of a triangular dst keep the masked
+//     register epilogue (the untouched triangle must not be written, not even with its own values).
+template <bool WIDE>
+struct Shape {
+  static constexpr int BN = WIDE ? 128 : 64;
+  static constexpr int CONSUMERS = WIDE ? 8 : 4;            // consumer warps: 4 along m x BN / 64 along n
+  static constexpr int THREADS = 128 + 32 * CONSUMERS;      // warpgroup 0: producer (warp 0 works), then the consumers
+  static constexpr int STAGES = WIDE ? 3 : 4;
+  static constexpr int B_BYTES = BN * BK * 8, STAGE_BYTES = A_BYTES + B_BYTES;
+  static constexpr int DST_BYTES = WIDE ? BM * BN * 8 : 0;  // 8 boxes of 16 rows x 128 columns, 128B-swizzled
+  static constexpr int SMEM_BYTES = DST_BYTES + STAGES * STAGE_BYTES + 1024 /*alignment*/ + 128 /*barriers*/;
+  // registers per thread after setmaxnreg; the launch gives every thread 65536 / THREADS (rounded down to a multiple of
+  // 8): 128 x 24 + 128 x 232 = 256 x 128, and 128 x 40 + 256 x 232 = 384 x 168
+  static constexpr int PRODUCER_REGS = WIDE ? 40 : 24, CONSUMER_REGS = 232;
+};
+static_assert(Shape<true>::SMEM_BYTES <= 227 * 1024, "wide configuration exceeds the shared memory of one SM");
+static_assert(128 * Shape<true>::PRODUCER_REGS + 256 * Shape<true>::CONSUMER_REGS <= 384 * 168, "register file");
 
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
@@ -77,10 +100,18 @@ __device__ __forceinline__ void tma_load_2d(uint32_t smem_dst, const CUtensorMap
       ::"r"(smem_dst), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t smem_src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(map), "r"(smem_src), "r"(c0), "r"(c1)
+               : "memory");
+}
 __device__ __forceinline__ double lds64(uint32_t addr) {
   double v;
   asm volatile("ld.shared.f64 %0, [%1];" : "=d"(v) : "r"(addr));
   return v;
+}
+__device__ __forceinline__ void sts64(uint32_t addr, double v) {
+  asm volatile("st.shared.f64 [%0], %1;" ::"r"(addr), "d"(v) : "memory");
 }
 
 struct Params {
@@ -88,6 +119,7 @@ struct Params {
   i64 c_rs, c_cs;
   int m, n, k;
   int c_struct, accum;
+  int dst_tma;  // wide configuration: the dst tensor map is valid, tiles inside the kept part go through shared memory
   double alpha;
   int tiles_m, tiles_n;
   int tiles_per_cta;
@@ -107,6 +139,7 @@ struct Params {
 // ---- static tile schedule: tile `idx` of the launch -> (tm, tn); identical in every warp of every CTA ---------------
 // RECT: grouped rasterisation (GROUP_M tile-rows share their lhs slabs through L2). Triangular dst: only the tiles that
 // intersect the kept triangle are enumerated (row-major over tile-rows), so the round-robin stays balanced.
+template <int BN>
 struct TileWalk {
   int tiles_m, tiles_n, c_struct;
   int row, row_first;  // triangular: current tile-row and the linear index of its first tile
@@ -162,14 +195,22 @@ __device__ __forceinline__ uint32_t off_k_major(int mn, int kk) {
 // through the async proxy: a write-after-read ACROSS proxies, which the mbarrier hand-over alone does not order. Without
 // `fence.proxy.async` before the arrive on `empty[s]`, a warp can read B fragments the next load has already replaced. The old values of dst are read with ld.global.cg:
 // they are used once, and keeping them out of L1 leaves it to nothing at all (the operands arrive by TMA).
-template <bool A_KMAJOR, bool B_KMAJOR, bool SPICY, int VAR = 0>
-__global__ void __launch_bounds__(THREADS, VAR == 1 ? 1 : 2)   // 128 registers per thread at launch, re-divided below
-gemm_f64_ws_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB, const Params p) {
+template <bool WIDE, bool A_KMAJOR, bool B_KMAJOR, bool SPICY, int VAR = 0>
+__global__ void __launch_bounds__(Shape<WIDE>::THREADS, (VAR == 1 || WIDE) ? 1 : 2)  // re-divided below with setmaxnreg
+gemm_f64_ws_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
+                   const __grid_constant__ CUtensorMap mapC, const Params p) {
+  using S = Shape<WIDE>;
+  constexpr int BN = S::BN, STAGES = S::STAGES, STAGE_BYTES = S::STAGE_BYTES, CONSUMERS = S::CONSUMERS;
+  static_assert(!(WIDE && (SPICY || VAR != 0)), "the wide configuration has no spicy or bring-up variants");
   extern __shared__ uint8_t ws_smem_raw[];
   const uint32_t smem_base = (smem_u32(ws_smem_raw) + 1023u) & ~1023u;
   uint8_t* smem_gen = ws_smem_raw + (smem_base - smem_u32(ws_smem_raw));
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem_gen + STAGES * STAGE_BYTES);
+  const uint32_t sdst = smem_base;                        // wide: destination tile buffer
+  const uint32_t sstages = smem_base + S::DST_BYTES;      // operand ring
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem_gen + S::DST_BYTES + STAGES * STAGE_BYTES);
   uint64_t* empty = full + STAGES;
+  uint64_t* dst_full = empty + STAGES;   // wide: old dst values landed (Add) / buffer free to overwrite (Replace)
+  uint64_t* dst_free = dst_full + 1;     // wide: the previous TMA store has read the buffer
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
@@ -177,27 +218,40 @@ gemm_f64_ws_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
       mbar_init(&full[s], 1);
       mbar_init(&empty[s], CONSUMERS);
     }
+    mbar_init(dst_full, 1);
+    mbar_init(dst_free, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
 
   const int nkt = (p.k + BK - 1) / BK;
-  TileWalk walk;
+  TileWalk<BN> walk;
   walk.init(p.tiles_m, p.tiles_n, p.c_struct);
+  // wide: does tile (tm, tn) lie wholly inside the kept part of dst (BM == BN, so off-diagonal tiles do)?
+  auto staged = [&](int tm, int tn) -> bool {
+    if constexpr (!WIDE) return false;
+    if (!p.dst_tma) return false;
+    if (is_lower(p.c_struct)) return tm > tn;
+    if (is_upper(p.c_struct)) return tn > tm;
+    return true;
+  };
 
   if (warp < 4) {
     // ================= producer warpgroup =================
-    if constexpr (VAR != 1) asm volatile("setmaxnreg.dec.sync.aligned.u32 24;");
+    if constexpr (VAR != 1) asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(S::PRODUCER_REGS));
     if (warp == 0 && lane == 0) {
       uint32_t it = 0;  // global k-step counter: stage = it % STAGES, phase = (it / STAGES) & 1
+      uint32_t ds = 0;  // staged tiles so far
       for (int i = 0; i < p.tiles_per_cta; ++i) {
         int tm, tn;
         if (!walk.locate((int)blockIdx.x * p.tiles_per_cta + i, tm, tn)) break;
         const int m0 = tm * BM, n0 = tn * BN;
+        const bool st = staged(tm, tn);
+        const int dst_at = min(STAGES, nkt) - 1;
         for (int kt = 0; kt < nkt; ++kt, ++it) {
           const uint32_t s = it % STAGES, ph = (it / STAGES) & 1u;
           mbar_wait(&empty[s], ph ^ 1u);
-          const uint32_t sa = smem_base + s * STAGE_BYTES, sb = sa + A_BYTES;
+          const uint32_t sa = sstages + s * STAGE_BYTES, sb = sa + A_BYTES;
           mbar_expect_tx(&full[s], STAGE_BYTES);
           const int k0 = kt * BK;
           if constexpr (A_KMAJOR) {
@@ -212,16 +266,30 @@ gemm_f64_ws_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
 #pragma unroll
             for (int b = 0; b < BN / 16; ++b) tma_load_2d(sb + b * 2048, &mapB, &full[s], n0 + b * 16, k0);
           }
+          // the old dst tile is requested once the ring holds this tile's first stages: waiting here for the previous
+          // tile's store costs nothing, since the next stage needs the consumers back in the main loop anyway
+          if (st && kt == dst_at) {
+            mbar_wait(dst_free, (ds & 1u) ^ 1u);
+            if (p.accum) {
+              mbar_expect_tx(dst_full, S::DST_BYTES);
+#pragma unroll
+              for (int b = 0; b < BM / 16; ++b) tma_load_2d(sdst + b * (16 * BN * 8), &mapC, dst_full, m0 + b * 16, n0);
+            } else {
+              mbar_arrive(dst_full);
+            }
+            ++ds;
+          }
         }
       }
     }
     return;
   }
 
-  // ================= consumer warpgroup =================
-  if constexpr (VAR != 1) asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+  // ================= consumer warpgroups =================
+  if constexpr (VAR != 1) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(S::CONSUMER_REGS));
+  const int cw = warp - 4;
   const int g = lane >> 2, t = lane & 3;
-  const int wm0 = (warp - 4) * (WMI * 8);  // warp tile rows [wm0, wm0 + 32) x all 64 columns
+  const int wm0 = (cw & 3) * (WMI * 8), wn0 = (cw >> 2) * (WNI * 8);  // warp tile rows [wm0, wm0 + 32) x cols [wn0, wn0 + 64)
   // per-lane fragment offsets for the 4 k slots of a stage: k index K4(q, t) = {0,3,12,15}[t] ^ {0,1,4,5}[q]
   uint32_t offA[4][2], offB[4][2];  // [k slot][parity of the 8-row block] (MN-major) / [k slot][0] (K-major)
   {
@@ -237,11 +305,11 @@ gemm_f64_ws_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
         offA[s][1] = off_mn_major(wm0 + 8 + g, kk);
       }
       if constexpr (B_KMAJOR) {
-        offB[s][0] = off_k_major(g, kk);
+        offB[s][0] = off_k_major(wn0 + g, kk);
         offB[s][1] = 0;
       } else {
-        offB[s][0] = off_mn_major(g, kk);
-        offB[s][1] = off_mn_major(8 + g, kk);
+        offB[s][0] = off_mn_major(wn0 + g, kk);
+        offB[s][1] = off_mn_major(wn0 + 8 + g, kk);
       }
     }
   }
@@ -252,12 +320,13 @@ gemm_f64_ws_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
   const double alpha = p.alpha;
   const bool add = p.accum != 0;
 
-  if (p.stagger_cycles > 0 && (int)blockIdx.x >= p.sm_slots && (int)blockIdx.x < 2 * p.sm_slots) {
+  if (!WIDE && p.stagger_cycles > 0 && (int)blockIdx.x >= p.sm_slots && (int)blockIdx.x < 2 * p.sm_slots) {
     const long long t0 = clock64();
     while (clock64() - t0 < p.stagger_cycles) __nanosleep(256);
   }
 
   uint32_t it = 0;
+  uint32_t dc = 0;  // staged tiles so far
   for (int ti = 0; ti < p.tiles_per_cta; ++ti) {
     int tm, tn;
     if (!walk.locate((int)blockIdx.x * p.tiles_per_cta + ti, tm, tn)) break;
@@ -283,7 +352,7 @@ gemm_f64_ws_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
         }
       }
       mbar_wait(&full[s], ph);
-      const uint32_t sa = smem_base + s * STAGE_BYTES, sb = sa + A_BYTES;
+      const uint32_t sa = sstages + s * STAGE_BYTES, sb = sa + A_BYTES;
       // two DMMA.16x8x8 per 16 x 8 block and stage (the 16-deep shape's fragments do not fit beside the 128 accumulator
       // registers): half h contracts fragment k slots q = 2h + (v >> 1) (A) / 2h + i (B), i.e. stage indices K4(q, t).
       // A fragments of the whole warp tile, B fragments one 8-column block at a time.
@@ -318,9 +387,42 @@ gemm_f64_ws_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
       if (lane == 0) mbar_arrive(&empty[s]);
     }
 
-    // ---- epilogue: dst = [dst +] alpha * acc, masked by dst structure and bounds. Add mode: the old values of row block
-    // i + 1 are requested before row block i is combined and stored (two register sets), so the four row blocks cost about
-    // two global-memory round trips instead of four ----
+    if (staged(tm, tn)) {
+      // ---- wide epilogue through shared memory: buffer = alpha * acc [+ old], then one TMA store of the tile. Element
+      // (r, c) of the tile sits in box r / 16 at line c, 16-byte chunk ((r & 15) / 2) ^ (c & 7): a half-warp's 8-byte
+      // accesses (4 rows x 4 column pairs) hit 16 distinct banks ----
+      mbar_wait(dst_full, dc & 1u);
+      ++dc;
+#pragma unroll
+      for (int i = 0; i < WMI; ++i) {
+        const int r = wm0 + i * 8 + g;
+        const uint32_t rbase = sdst + (r >> 4) * (16 * BN * 8) + ((r & 1) << 3);
+        const int rchunk = (r & 15) >> 1;
+#pragma unroll
+        for (int j = 0; j < WNI; ++j)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int c = wn0 + j * 8 + 2 * t + e;
+            const uint32_t addr = rbase + c * 128 + ((rchunk ^ (c & 7)) << 4);
+            sts64(addr, add ? (alpha * acc[i][j][e] + lds64(addr)) : alpha * acc[i][j][e]);
+          }
+      }
+      // the generic-proxy writes above must be visible to the async proxy (the TMA store) before it reads the buffer
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+      asm volatile("bar.sync 1, %0;" ::"n"(CONSUMERS * 32) : "memory");
+      if (cw == 0 && lane == 0) {
+#pragma unroll
+        for (int b = 0; b < BM / 16; ++b) tma_store_2d(&mapC, sdst + b * (16 * BN * 8), m0 + b * 16, n0);
+        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+        asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+        mbar_arrive(dst_free);
+      }
+      continue;
+    }
+
+    // ---- register epilogue: dst = [dst +] alpha * acc, masked by dst structure and bounds. Add mode: the old values of
+    // row block i + 1 are requested before row block i is combined and stored (two register sets), so the four row blocks
+    // cost about two global-memory round trips instead of four ----
     auto coloff = [&](int col) -> i64 {
       if constexpr (SPICY) {
         if (p.col_idx) return col < p.n ? (i64)p.col_idx[col] * p.c_cs : 0;
@@ -347,7 +449,7 @@ gemm_f64_ws_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
       for (int j = 0; j < WNI; ++j)
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
-          const int col = n0 + j * 8 + 2 * t + e;
+          const int col = n0 + wn0 + j * 8 + 2 * t + e;
           if constexpr (VAR != 5) dst[j][e] = kept(row, col) ? __ldcg(p.C + roff + coloff(col)) : 0.0;
           else dst[j][e] = kept(row, col) ? p.C[roff + coloff(col)] : 0.0;
         }
@@ -362,12 +464,14 @@ gemm_f64_ws_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
       for (int j = 0; j < WNI; ++j) {
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
-          const int col = n0 + j * 8 + 2 * t + e;
+          const int col = n0 + wn0 + j * 8 + 2 * t + e;
           if (kept(row, col)) p.C[roff + coloff(col)] = add ? (alpha * acc[i][j][e] + cv[i & 1][j][e]) : alpha * acc[i][j][e];
         }
       }
     }
   }
+  // the tile stores must have completed before the kernel ends
+  if (WIDE && cw == 0 && lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -410,21 +514,37 @@ inline bool tma_layout(const double* ptr, i64 rows, i64 k, i64 s_mn, i64 s_k, bo
   return false;
 }
 
-// Launches the kernel if the problem qualifies; returns false otherwise (caller falls back to the cp.async kernel).
 struct Spicy {
   const long long* row_idx = nullptr;
   const long long* col_idx = nullptr;
   const double* diag = nullptr;
   i64 diag_stride = 1;
 };
-inline bool try_gemm_f64_ws(cudaStream_t stream, const GemmF64Params& q, const Spicy* sp = nullptr) {
-  if (q.a_struct != RECT || q.b_struct != RECT || q.k_split_len > 0) return false;
+// tiles the kernel enumerates for an m x n dst of structure c_struct with CTA tiles BM x bn (see TileWalk)
+inline long long ws_tiles(int m, int n, int c_struct, int bn) {
+  const int tiles_m = (m + BM - 1) / BM, tiles_n = (n + bn - 1) / bn;
+  if (c_struct == RECT) return (long long)tiles_m * tiles_n;
+  long long tiles = 0;
+  for (int tm = 0; tm < tiles_m; ++tm) {
+    const int lo = is_upper(c_struct) ? (tm * BM) / bn : 0;
+    const int hi = is_lower(c_struct) ? std::min(tiles_n, (tm * BM + BM - 1) / bn + 1) : tiles_n;
+    tiles += std::max(0, hi - lo);
+  }
+  return tiles;
+}
+
+// Launches the kernel if the problem qualifies; returns false otherwise (caller falls back to the cp.async kernel).
+// `wide` selects the 128 x 128 configuration (no spicy variant).
+inline bool try_gemm_f64_ws(cudaStream_t stream, const GemmF64Params& q, const Spicy* sp = nullptr, bool wide = false) {
+  if (q.a_struct != RECT || q.b_struct != RECT || q.k_split_len > 0 || q.k < 1) return false;
+  if (wide && sp) return false;
   if (!encode_fn()) return false;
   bool ak = false, bk = false;
   if (!tma_layout(q.A, q.m, q.k, q.a_rs, q.a_cs, &ak)) return false;
   if (!tma_layout(q.B, q.n, q.k, q.b_cs, q.b_rs, &bk)) return false;
   if (q.a_rs == 1 && q.a_cs == 1) return false;  // degenerate vectors: leave to the general kernel
   if (q.b_rs == 1 && q.b_cs == 1) return false;
+  const int bn = wide ? Shape<true>::BN : Shape<false>::BN;
   Params p;
   p.C = q.C; p.c_rs = q.c_rs; p.c_cs = q.c_cs;
   p.m = q.m; p.n = q.n; p.k = q.k;
@@ -434,26 +554,38 @@ inline bool try_gemm_f64_ws(cudaStream_t stream, const GemmF64Params& q, const S
   p.diag = sp ? sp->diag : nullptr;
   p.diag_stride = sp ? sp->diag_stride : 1;
   p.tiles_m = (q.m + BM - 1) / BM;
-  p.tiles_n = (q.n + BN - 1) / BN;
-  long long tiles = (long long)p.tiles_m * p.tiles_n;
-  if (q.c_struct != RECT) {  // exactly the tiles TileWalk enumerates
-    tiles = 0;
-    for (int tm = 0; tm < p.tiles_m; ++tm) {
-      const int lo = is_upper(q.c_struct) ? (tm * BM) / BN : 0;
-      const int hi = is_lower(q.c_struct) ? std::min(p.tiles_n, (tm * BM + BM - 1) / BN + 1) : p.tiles_n;
-      tiles += std::max(0, hi - lo);
+  p.tiles_n = (q.n + bn - 1) / bn;
+  const long long tiles = ws_tiles(q.m, q.n, q.c_struct, bn);
+  if (tiles == 0) return true;
+  CUtensorMap mapA, mapB, mapC;
+  const bool okA = ak ? make_map(&mapA, q.A, q.k, q.m, q.a_rs, BM) : make_map(&mapA, q.A, q.m, q.k, q.a_cs, 16);
+  const bool okB = bk ? make_map(&mapB, q.B, q.k, q.n, q.b_cs, bn) : make_map(&mapB, q.B, q.n, q.k, q.b_rs, 16);
+  if (!okA || !okB) return false;
+  // wide: dst tiles through shared memory when TMA can address dst (column-major, 16-byte aligned base and ld); any other
+  // dst takes the register epilogue for every tile
+  p.dst_tma = wide && q.c_rs == 1 && q.c_cs >= q.m && q.c_cs % 2 == 0 && (((uintptr_t)q.C) & 15) == 0 &&
+              make_map(&mapC, q.C, q.m, q.n, q.c_cs, 128);
+  if (!p.dst_tma) mapC = mapA;  // not read
+  p.sm_slots = stream_sms(stream);
+  if (!wide) {
+    // tiles per CTA shrink with k so that a CTA stays short-lived (on the order of 50 us at 128 f64 FMA / clock / SM), and
+    // never below two CTAs per SM while the tiles allow it (fewer would leave SMs idle in small launches)
+    const long long tpc_fill = std::max<long long>(1, (tiles + 2ll * p.sm_slots - 1) / (2ll * p.sm_slots));
+    p.tiles_per_cta = (int)std::max<long long>(1, std::min<long long>({8, 768 / std::max(q.k, 1), tpc_fill}));
+  } else {
+    // one CTA per SM, so a launch takes ceil(CTAs / SMs) waves of tiles_per_cta tiles. Up to 1024 / k tiles per CTA
+    // (about 70 us at k = 256 and the full DMMA rate: long enough to amortise the pipeline fill and the last tile's
+    // store, short enough that the SMs turn over for the panel stream of the look-ahead factorizations); among those,
+    // the count with the shortest launch, each CTA start charged 0.15 tile
+    const int tpc_max = (int)std::max<long long>(1, std::min<long long>(8, 1024 / q.k));
+    double best = 1e300;
+    p.tiles_per_cta = 1;
+    for (int tpc = 1; tpc <= tpc_max; ++tpc) {
+      const long long waves = ((tiles + tpc - 1) / tpc + p.sm_slots - 1) / p.sm_slots;
+      const double cost = (double)waves * (tpc + 0.15);
+      if (cost < best) { best = cost; p.tiles_per_cta = tpc; }
     }
   }
-  if (tiles == 0) return true;
-  CUtensorMap mapA, mapB;
-  const bool okA = ak ? make_map(&mapA, q.A, q.k, q.m, q.a_rs, BM) : make_map(&mapA, q.A, q.m, q.k, q.a_cs, 16);
-  const bool okB = bk ? make_map(&mapB, q.B, q.k, q.n, q.b_cs, BN) : make_map(&mapB, q.B, q.n, q.k, q.b_rs, 16);
-  if (!okA || !okB) return false;
-  // tiles per CTA shrink with k so that a CTA stays short-lived (on the order of 50 us at 128 f64 FMA / clock / SM), and
-  // never below two CTAs per SM while the tiles allow it (fewer would leave SMs idle in small launches)
-  p.sm_slots = stream_sms(stream);
-  const long long tpc_fill = std::max<long long>(1, (tiles + 2ll * p.sm_slots - 1) / (2ll * p.sm_slots));
-  p.tiles_per_cta = (int)std::max<long long>(1, std::min<long long>({8, 768 / std::max(q.k, 1), tpc_fill}));
   const int grid = (int)((tiles + p.tiles_per_cta - 1) / p.tiles_per_cta);
   {
     static int stagger = -1;
@@ -461,11 +593,12 @@ inline bool try_gemm_f64_ws(cudaStream_t stream, const GemmF64Params& q, const S
       const char* e = getenv("FAER_B200_WS_STAGGER");  // 0 switches the stagger off (dev knob)
       stagger = e ? atoi(e) : 1;
     }
-    // half a tile at the full rate of one SM: (k / 16) k-steps x 128 x 64 x 16 FMA / (128 FMA / clock) / 2
-    p.stagger_cycles = (stagger && grid >= 2 * p.sm_slots) ? (long long)((q.k + BK - 1) / BK) * 512 : 0;
+    // narrow only (two CTAs per SM): half a tile at the full rate of one SM, (k / 16) k-steps x 128 x 64 x 16 FMA /
+    // (128 FMA / clock) / 2
+    p.stagger_cycles = (!wide && stagger && grid >= 2 * p.sm_slots) ? (long long)((q.k + BK - 1) / BK) * 512 : 0;
   }
   // one opt-in to > 48 KB of dynamic shared memory per kernel variant
-  static bool configured[16] = {};
+  static bool configured[20] = {};
   static int var = -1, extra_smem = 0;
   if (var < 0) {
     const char* e = getenv("FAER_B200_WS_VAR");  // bring-up knob
@@ -473,27 +606,34 @@ inline bool try_gemm_f64_ws(cudaStream_t stream, const GemmF64Params& q, const S
     const char* x = getenv("FAER_B200_WS_EXTRA_SMEM");  // bring-up knob: > 14 KB forces one CTA per SM
     extra_smem = x ? atoi(x) : 0;
   }
-  const int smem_bytes = SMEM_BYTES + extra_smem;
-  auto launch = [&](int which, void (*kern)(CUtensorMap, CUtensorMap, Params)) {
+  auto launch = [&](int which, auto kern, int threads, int smem_bytes) {
     if (!configured[which]) {
       FB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
       configured[which] = true;
     }
-    kern<<<grid, THREADS, smem_bytes, stream>>>(mapA, mapB, p);
+    kern<<<grid, threads, smem_bytes, stream>>>(mapA, mapB, mapC, p);
   };
-  if (!sp && var != 0 && !ak) {
-    if (var == 1) { if (bk) launch(8, gemm_f64_ws_kernel<false, true, false, 1>); else launch(9, gemm_f64_ws_kernel<false, false, false, 1>); }
-    else { if (bk) launch(10, gemm_f64_ws_kernel<false, true, false, 5>); else launch(11, gemm_f64_ws_kernel<false, false, false, 5>); }
+  using N = Shape<false>;
+  using W = Shape<true>;
+  const int nsm = N::SMEM_BYTES + extra_smem;
+  if (wide) {
+    if (ak && bk) launch(16, gemm_f64_ws_kernel<true, true, true, false>, W::THREADS, W::SMEM_BYTES);
+    else if (ak && !bk) launch(17, gemm_f64_ws_kernel<true, true, false, false>, W::THREADS, W::SMEM_BYTES);
+    else if (!ak && bk) launch(18, gemm_f64_ws_kernel<true, false, true, false>, W::THREADS, W::SMEM_BYTES);
+    else launch(19, gemm_f64_ws_kernel<true, false, false, false>, W::THREADS, W::SMEM_BYTES);
+  } else if (!sp && var != 0 && !ak) {
+    if (var == 1) { if (bk) launch(8, gemm_f64_ws_kernel<false, false, true, false, 1>, N::THREADS, nsm); else launch(9, gemm_f64_ws_kernel<false, false, false, false, 1>, N::THREADS, nsm); }
+    else { if (bk) launch(10, gemm_f64_ws_kernel<false, false, true, false, 5>, N::THREADS, nsm); else launch(11, gemm_f64_ws_kernel<false, false, false, false, 5>, N::THREADS, nsm); }
   } else if (!sp) {
-    if (ak && bk) launch(0, gemm_f64_ws_kernel<true, true, false>);
-    else if (ak && !bk) launch(1, gemm_f64_ws_kernel<true, false, false>);
-    else if (!ak && bk) launch(2, gemm_f64_ws_kernel<false, true, false>);
-    else launch(3, gemm_f64_ws_kernel<false, false, false>);
+    if (ak && bk) launch(0, gemm_f64_ws_kernel<false, true, true, false>, N::THREADS, nsm);
+    else if (ak && !bk) launch(1, gemm_f64_ws_kernel<false, true, false, false>, N::THREADS, nsm);
+    else if (!ak && bk) launch(2, gemm_f64_ws_kernel<false, false, true, false>, N::THREADS, nsm);
+    else launch(3, gemm_f64_ws_kernel<false, false, false, false>, N::THREADS, nsm);
   } else {
-    if (ak && bk) launch(4, gemm_f64_ws_kernel<true, true, true>);
-    else if (ak && !bk) launch(5, gemm_f64_ws_kernel<true, false, true>);
-    else if (!ak && bk) launch(6, gemm_f64_ws_kernel<false, true, true>);
-    else launch(7, gemm_f64_ws_kernel<false, false, true>);
+    if (ak && bk) launch(4, gemm_f64_ws_kernel<false, true, true, true>, N::THREADS, nsm);
+    else if (ak && !bk) launch(5, gemm_f64_ws_kernel<false, true, false, true>, N::THREADS, nsm);
+    else if (!ak && bk) launch(6, gemm_f64_ws_kernel<false, false, true, true>, N::THREADS, nsm);
+    else launch(7, gemm_f64_ws_kernel<false, false, false, true>, N::THREADS, nsm);
   }
   FB_CUDA_CHECK(cudaGetLastError());
   note_launch();

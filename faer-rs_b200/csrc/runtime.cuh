@@ -24,6 +24,7 @@ bool is_device_pointer(const void* p);
 // those). Persistent kernels size their grids with it.
 // Run-time options (C ABI: faer_b200_set_option / faer_b200_get_option; initial values from the environment):
 //   gemm_ws        FAER_B200_GEMM_WS        0 = never use the TMA / warp-specialised f64 GEMM, 1 = heuristic (default), 2 = always
+//                                           (128 x 64 tiles), 3 = always (128 x 128 tiles)
 //   f64_gemm_mode  FAER_B200_F64_GEMM_MODE  0 = native f64 tensor op (DMMA; default), 1 = int8-sliced wgmma products for  
 //                                           large unstructured `matmul`s (opt-in; accuracy contract in gemm_f64_sliced.cuh)
 enum Option : int { OPT_GEMM_WS = 0, OPT_F64_GEMM_MODE = 1, OPT_COUNT };

@@ -647,7 +647,8 @@ void faer_b200_gemm(int dtype, int itype, int instr_set, size_t m, size_t n, siz
                     ptrdiff_t rhs_rs, ptrdiff_t rhs_cs, bool conj_rhs, const void *alpha, size_t n_threads);
 /* Run-time options (initial values from the environment variable in brackets). Returns 0, or -1 for an unknown name.
  *   "gemm_ws"        [FAER_B200_GEMM_WS]        0 never / 1 heuristic (default) / 2 always use the TMA-fed warp-specialised
- *                                                f64 GEMM (csrc/gemm_f64_ws.cuh) where the operands qualify
+ *                                                f64 GEMM (csrc/gemm_f64_ws.cuh) where the operands qualify, 128 x 64 tiles /
+ *                                                3 always, 128 x 128 tiles (spicy_matmul: as 1)
  *   "f64_gemm_mode"  [FAER_B200_F64_GEMM_MODE]  0 native f64 tensor op (default) / 1 int8-sliced wgmma products for large  
  *                                                unstructured matmuls (csrc/gemm_f64_sliced.cuh states the accuracy contract) */
 int faer_b200_set_option(const char *name, long long value);

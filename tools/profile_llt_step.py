@@ -1,11 +1,13 @@
 """Per-kernel breakdown of ONE f64 LLT step of the headline workload (n = 16384, bench.py's input and call) with
 torch.profiler: device time per kernel name, summed over the step; how much of the step no kernel covers (exposed gaps);
-and the largest trailing update (lower-triangular n = 16128, k = 256) timed on its own with CUDA events.
+per CUDA stream (the look-ahead driver's bulk-update stream and its high-priority panel stream), the busy time and the
+kernel time per name, and the wall time during which only the panel stream is busy; and the largest trailing update (lower-triangular n = 16128, k = 256) timed on its own with CUDA events.
 usage: python tools/profile_llt_step.py [out_dir]   (writes out_dir/llt_step_profile.json)"""
 import json
 import os
 import re
 import sys
+import tempfile
 
 import torch
 from torch.profiler import ProfilerActivity, profile
@@ -57,6 +59,60 @@ for e in kernels:
     d["launches"] += 1
 per = dict(sorted(per.items(), key=lambda kv: -kv[1]["ms"]))
 
+
+def union(iv):
+    out = []
+    for s, e in sorted(iv):
+        if out and s <= out[-1][1]:
+            out[-1][1] = max(out[-1][1], e)
+        else:
+            out.append([s, e])
+    return out
+
+
+# per-stream split from the trace (the stream id is only exported there)
+with tempfile.TemporaryDirectory() as td:
+    path = os.path.join(td, "trace.json")
+    prof.export_chrome_trace(path)
+    with open(path) as fh:
+        trace = json.load(fh)
+streams = {}
+for ev in trace.get("traceEvents", []):
+    if ev.get("cat") != "kernel":
+        continue
+    st = ev.get("args", {}).get("stream")
+    m = re.search(r"(\w+_kernel)\b", ev["name"])
+    name = m.group(1) if m else ev["name"][:80]
+    d = streams.setdefault(st, {"iv": [], "kernels": {}})
+    d["iv"].append((ev["ts"], ev["ts"] + ev["dur"]))
+    k = d["kernels"].setdefault(name, {"ms": 0.0, "launches": 0})
+    k["ms"] += ev["dur"] / 1e3
+    k["launches"] += 1
+# the bulk stream is the one with the most gemm time; any other stream counts as the panel chain
+by_gemm = sorted(streams, key=lambda s: -streams[s]["kernels"].get("gemm_f64_ws_kernel", {"ms": 0})["ms"]
+                 - streams[s]["kernels"].get("gemm_f64_kernel", {"ms": 0})["ms"])
+per_stream = {}
+if by_gemm:
+    bulk = union(streams[by_gemm[0]]["iv"])
+    panel = union([iv for s in by_gemm[1:] for iv in streams[s]["iv"]])
+    # wall time in which the panel streams are busy and the bulk stream is not
+    only_panel = 0.0
+    for s, e in panel:
+        cur = s
+        for bs, be in bulk:
+            if be <= cur or bs >= e:
+                continue
+            if bs > cur:
+                only_panel += bs - cur
+            cur = max(cur, be)
+        if cur < e:
+            only_panel += e - cur
+    for i, s in enumerate(by_gemm):
+        per_stream[f"{'bulk' if i == 0 else 'panel'}_stream_{s}"] = {
+            "busy_ms": sum(e - b for b, e in union(streams[s]["iv"])) / 1e3,
+            "kernels": dict(sorted(streams[s]["kernels"].items(), key=lambda kv: -kv[1]["ms"]))}
+    per_stream["only_panel_busy_ms"] = only_panel / 1e3
+
 # the largest trailing update on its own: dst(lower, 16128^2) -= P P^T, P 16128 x 256 (the shape of the first block step)
 m, k = n - 256, 256
 P = torch.randn((k, m), dtype=torch.float64, device=dev).T
@@ -69,7 +125,7 @@ for _ in range(10):
     e0.record(); f(); e1.record(); torch.cuda.synchronize()
     best = min(best, e0.elapsed_time(e1))
 res = {"n": n, "step_ms": (t1 - t0) / 1e3, "kernel_busy_ms": busy / 1e3, "exposed_gap_ms": (t1 - t0 - busy) / 1e3,
-       "kernels": per,
+       "kernels": per, "streams": per_stream,
        "largest_update": {"m": m, "k": k, "ms": best, "tflops": m * (m + 1.0) * k / (best * 1e-3) / 1e12}}
 print(json.dumps(res, indent=1))
 os.makedirs(out_dir, exist_ok=True)

@@ -1,4 +1,5 @@
-"""Dev aid: the ws f64 GEMM (gemm_ws = 2) against the cp.async kernel (0) on the trailing-update shapes of LLT / LU.
+"""Dev aid: the ws f64 GEMM, narrow (gemm_ws = 2, 128 x 64 tiles) and wide (3, 128 x 128 tiles), against the cp.async kernel
+(0) on the trailing-update shapes of LLT / LU.
 usage: [FAER_B200_WS_STAGGER=0|1] python tools/time_ws_shapes.py"""
 import os
 import sys
@@ -28,7 +29,7 @@ for (n, k) in [(16128, 256), (12288, 256), (8192, 256), (4096, 256), (1024, 256)
     P = torch.randn((k, n), dtype=torch.float64, device=dev).T
     Cm = torch.randn((n, n), dtype=torch.float64, device=dev).T
     line = f"{tag} SYRK(lower) n={n} k={k}:"
-    for mode in (0, 2):
+    for mode in (0, 2, 3):
         lib.faer_b200_set_option(b"gemm_ws", mode)
         ms = best(lambda: la.matmul_triangular(Cm, 1, 1, P, 0, P.T, 0, -1.0))
         line += f"  mode {mode}: {ms:.3f} ms {n * n * k / ms / 1e9:.2f} TF"
@@ -41,7 +42,7 @@ for (m, n, k) in [(16384, 16384, 256), (16384, 16384, 512), (8192, 8192, 512), (
     U = torch.randn((n, k), dtype=torch.float64, device=dev).T
     Cm = torch.randn((n, m), dtype=torch.float64, device=dev).T
     line = f"{tag} update m={m} n={n} k={k}:"
-    for mode in (0, 2):
+    for mode in (0, 2, 3):
         lib.faer_b200_set_option(b"gemm_ws", mode)
         ms = best(lambda: la.matmul(Cm, 1, L, U, -1.0))
         line += f"  mode {mode}: {ms:.3f} ms {2.0 * m * n * k / ms / 1e9:.2f} TF"
