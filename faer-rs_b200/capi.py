@@ -135,6 +135,25 @@ class QrStatus(C.Structure):
     _fields_ = [("tag", C.c_int), ("body", _StatusBody)]
 
 
+class PivLltParams(C.Structure):
+    """faer.h:178-180."""
+    _fields_ = [("block_size", C.c_size_t)]
+
+
+class _PivLltOkBody(C.Structure):
+    _fields_ = [("rank", C.c_size_t), ("transposition_count", C.c_size_t)]
+
+
+class _PivLltBody(C.Union):
+    _fields_ = [("ok", _PivLltOkBody), ("index", C.c_size_t)]
+
+
+class PivLltStatus(C.Structure):
+    """tag: 0 Ok{rank, transposition_count}, 1 NonPositivePivot{index}, 2 Unknown (faer.h:432-453); 24 bytes, body at 8."""
+    _anonymous_ = ("body",)
+    _fields_ = [("tag", C.c_int), ("body", _PivLltBody)]
+
+
 ACCUM_REPLACE, ACCUM_ADD = 0, 1
 CONJ_NO, CONJ_YES = 0, 1
 PAR_SEQ, PAR_RAYON = 0, 1
@@ -376,6 +395,29 @@ def load() -> C.CDLL:
     lib.faer_b200_set_option.restype = C.c_int
     lib.faer_b200_get_option.argtypes = [C.c_char_p]
     lib.faer_b200_get_option.restype = C.c_longlong
+    for suf in ("f64", "f32", "c64", "c32"):
+        getattr(lib, f"libfaer_v0_23_PivLltParams_{suf}").argtypes = []
+        getattr(lib, f"libfaer_v0_23_PivLltParams_{suf}").restype = PivLltParams
+        for it in ("u32", "u64"):
+            f = getattr(lib, f"libfaer_v0_23_piv_llt_factor_in_place_scratch_{it}_{suf}")
+            f.argtypes = [C.c_size_t, P, PivLltParams]
+            f.restype = Layout
+            f = getattr(lib, f"libfaer_v0_23_piv_llt_factor_in_place_{it}_{suf}")
+            f.argtypes = [MatMut, SliceMut, SliceMut, P, MemAlloc, PivLltParams]
+            f.restype = PivLltStatus
+            f = getattr(lib, f"libfaer_v0_23_piv_llt_solve_in_place_scratch_{it}_{suf}")
+            f.argtypes = [C.c_size_t, C.c_size_t, P]
+            f.restype = Layout
+            f = getattr(lib, f"libfaer_v0_23_piv_llt_solve_in_place_{it}_{suf}")
+            f.argtypes = [MatRef, SliceMut, SliceMut, C.c_int, MatMut, P, MemAlloc]
+            f.restype = None
+            for name in ("reconstruct", "inverse"):
+                f = getattr(lib, f"libfaer_v0_23_piv_llt_{name}_scratch_{it}_{suf}")
+                f.argtypes = [C.c_size_t, P]
+                f.restype = Layout
+                f = getattr(lib, f"libfaer_v0_23_piv_llt_{name}_{it}_{suf}")
+                f.argtypes = [MatMut, MatRef, SliceMut, SliceMut, P, MemAlloc]
+                f.restype = None
     lib.faer_b200_version.argtypes = []
     lib.faer_b200_version.restype = C.c_char_p
     _lib = lib

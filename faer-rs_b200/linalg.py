@@ -708,3 +708,66 @@ def lu_in_place(A, perm, perm_inv, par=None, params=None) -> PartialPivLuInfo:
     if st.tag != 0:
         raise RuntimeError("PartialPivLuStatus::Unknown")
     return PartialPivLuInfo(int(st.value))
+
+
+# ---- pivoted Cholesky (llt_pivoting) ---------------------------------------------------------------
+@dataclass
+class PivLltInfo:
+    rank: int
+    transposition_count: int
+
+
+def piv_llt_params_default():
+    return capi.load().libfaer_v0_23_PivLltParams_f64()
+
+
+def _perm_width(perm) -> str:
+    isz = perm.element_size() if capi._is_torch(perm) else perm.itemsize
+    return {4: "u32", 8: "u64"}[isz]
+
+
+def piv_llt_in_place(A, perm, perm_inv, par=None, params=None) -> PivLltInfo:
+    """cholesky::llt_pivoting::factor::cholesky_in_place (llt_pivoting/factor.rs:47-199): P A P^T = L L^H of the lower triangle
+    of a positive semi-definite A, in place. `perm`/`perm_inv`: uint32/uint64 arrays (numpy) or int32/int64 CUDA tensors of
+    length n; (P A P^T)[i, j] = A[perm[i], perm[j]]. Returns the numerical rank: columns 0..rank of L are the factor. Raises
+    LltError(index) for a negative or NaN diagonal (index 0, A untouched) or a NaN residual (its column)."""
+    lib = capi.load()
+    suf = _suf_lu(A)
+    params = params or getattr(lib, f"libfaer_v0_23_PivLltParams_{suf}")()
+    par = par or capi.par_default()
+    it = _perm_width(perm)
+    lay = getattr(lib, f"libfaer_v0_23_piv_llt_factor_in_place_scratch_{it}_{suf}")(A.shape[0], par, params)
+    scratch = np.empty(lay.len_bytes + lay.align_bytes, dtype=np.uint8)
+    st = getattr(lib, f"libfaer_v0_23_piv_llt_factor_in_place_{it}_{suf}")(
+        capi.mat_mut(A), capi.slice_mut(perm), capi.slice_mut(perm_inv), par,
+        capi.MemAlloc(scratch.ctypes.data, scratch.size), params)
+    if st.tag == 0:
+        return PivLltInfo(int(st.ok.rank), int(st.ok.transposition_count))
+    if st.tag == 1:
+        raise LltError(int(st.index))
+    raise RuntimeError("PivLltStatus::Unknown")
+
+
+def piv_llt_solve_in_place(L, perm, perm_inv, rhs, conj: int = CONJ_NO, par=None) -> None:
+    """cholesky::llt_pivoting::solve::solve_in_place_with_conj (llt_pivoting/solve.rs:13-41): rhs <- A^-1 rhs (conj(A)^-1 rhs
+    with CONJ_YES) from the factor and its permutation."""
+    suf = _same_suffix(L, rhs)
+    getattr(capi.load(), f"libfaer_v0_23_piv_llt_solve_in_place_{_perm_width(perm)}_{suf}")(
+        capi.mat_ref(L), capi.slice_mut(perm), capi.slice_mut(perm_inv), conj, capi.mat_mut(rhs), par or capi.par_default(),
+        capi.MemAlloc(None, 0))
+
+
+def piv_llt_reconstruct(out, L, perm, perm_inv, par=None) -> None:
+    """cholesky::llt_pivoting::reconstruct (reconstruct.rs:12-52): the LOWER triangle of out <- A from the factor."""
+    suf = _same_suffix(out, L)
+    getattr(capi.load(), f"libfaer_v0_23_piv_llt_reconstruct_{_perm_width(perm)}_{suf}")(
+        capi.mat_mut(out), capi.mat_ref(L), capi.slice_mut(perm), capi.slice_mut(perm_inv), par or capi.par_default(),
+        capi.MemAlloc(None, 0))
+
+
+def piv_llt_inverse(out, L, perm, perm_inv, par=None) -> None:
+    """cholesky::llt_pivoting::inverse (inverse.rs:12-54): the LOWER triangle of out <- A^-1 from the factor."""
+    suf = _same_suffix(out, L)
+    getattr(capi.load(), f"libfaer_v0_23_piv_llt_inverse_{_perm_width(perm)}_{suf}")(
+        capi.mat_mut(out), capi.mat_ref(L), capi.slice_mut(perm), capi.slice_mut(perm_inv), par or capi.par_default(),
+        capi.MemAlloc(None, 0))

@@ -710,4 +710,8 @@ void libfaer_v0_23_partial_piv_lu_solve_transpose_in_place_u64_c32(struct FaerV0
 #ifdef __cplusplus
 }
 #endif
+
+/* pivoted Cholesky (piv_llt_*): declared in its own header */
+#include "faer_b200_piv_llt.h"
+
 #endif /* LIBFAER_V0_24 */
