@@ -154,6 +154,25 @@ class PivLltStatus(C.Structure):
     _fields_ = [("tag", C.c_int), ("body", _PivLltBody)]
 
 
+class ColPivQrParams(C.Structure):
+    """faer.h:101-104."""
+    _fields_ = [("blocking_threshold", C.c_size_t), ("par_threshold", C.c_size_t)]
+
+
+class _ColPivQrOkBody(C.Structure):
+    _fields_ = [("transposition_count", C.c_size_t)]
+
+
+class _ColPivQrBody(C.Union):
+    _fields_ = [("ok", _ColPivQrOkBody)]
+
+
+class ColPivQrStatus(C.Structure):
+    """tag: 0 Ok{transposition_count}, 1 Unknown (faer.h:234-248); 16 bytes, body at 8."""
+    _anonymous_ = ("body",)
+    _fields_ = [("tag", C.c_int), ("body", _ColPivQrBody)]
+
+
 ACCUM_REPLACE, ACCUM_ADD = 0, 1
 CONJ_NO, CONJ_YES = 0, 1
 PAR_SEQ, PAR_RAYON = 0, 1
@@ -417,6 +436,38 @@ def load() -> C.CDLL:
                 f.restype = Layout
                 f = getattr(lib, f"libfaer_v0_23_piv_llt_{name}_{it}_{suf}")
                 f.argtypes = [MatMut, MatRef, SliceMut, SliceMut, P, MemAlloc]
+                f.restype = None
+    for suf in ("f64", "f32", "c64", "c32"):
+        getattr(lib, f"libfaer_v0_23_ColPivQrParams_{suf}").argtypes = []
+        getattr(lib, f"libfaer_v0_23_ColPivQrParams_{suf}").restype = ColPivQrParams
+        for it in ("u32", "u64"):
+            pre = f"libfaer_v0_23_colpiv_qr_"
+            f = getattr(lib, f"{pre}factor_in_place_scratch_{it}_{suf}")
+            f.argtypes = [C.c_size_t, C.c_size_t, C.c_size_t, P, ColPivQrParams]
+            f.restype = Layout
+            f = getattr(lib, f"{pre}factor_in_place_{it}_{suf}")
+            f.argtypes = [MatMut, MatMut, SliceMut, SliceMut, P, MemAlloc, ColPivQrParams]
+            f.restype = ColPivQrStatus
+            for name in ("solve", "solve_transpose"):
+                f = getattr(lib, f"{pre}{name}_in_place_scratch_{it}_{suf}")
+                f.argtypes = [C.c_size_t, C.c_size_t, C.c_size_t, P]
+                f.restype = Layout
+            f = getattr(lib, f"{pre}solve_lstsq_in_place_scratch_{it}_{suf}")
+            f.argtypes = [C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, P]
+            f.restype = Layout
+            for name in ("solve", "solve_transpose", "solve_lstsq"):
+                f = getattr(lib, f"{pre}{name}_in_place_{it}_{suf}")
+                f.argtypes = [MatRef, MatRef, MatRef, C.c_int, SliceMut, SliceMut, MatMut, P, MemAlloc]
+                f.restype = None
+            f = getattr(lib, f"{pre}reconstruct_scratch_{it}_{suf}")
+            f.argtypes = [C.c_size_t, C.c_size_t, C.c_size_t, P]
+            f.restype = Layout
+            f = getattr(lib, f"{pre}inverse_scratch_{it}_{suf}")
+            f.argtypes = [C.c_size_t, C.c_size_t, P]
+            f.restype = Layout
+            for name in ("reconstruct", "inverse"):
+                f = getattr(lib, f"{pre}{name}_{it}_{suf}")
+                f.argtypes = [MatMut, MatRef, MatRef, MatRef, SliceMut, SliceMut, P, MemAlloc]
                 f.restype = None
     lib.faer_b200_version.argtypes = []
     lib.faer_b200_version.restype = C.c_char_p

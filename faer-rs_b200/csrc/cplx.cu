@@ -926,4 +926,11 @@ FB_CPLX_EXPORTS(c64, double)
 FB_CPLX_EXPORTS(c32, float)
 #undef FB_CPLX_EXPORTS
 
+template <class R>
+void householder_build_t_cx(cudaStream_t st, View<const R> V, View<R> Tf) {
+  upgrade_householder_factor_cx<R>(st, Tf, V, Tf.nrows, 1);
+}
+template void householder_build_t_cx<double>(cudaStream_t, View<const double>, View<double>);
+template void householder_build_t_cx<float>(cudaStream_t, View<const float>, View<float>);
+
 }  // namespace fb

@@ -276,4 +276,13 @@ FB_RECON_INST(double, true)
 FB_RECON_INST(float, true)
 #undef FB_RECON_INST
 
+template <class R, bool CX>
+void permute_rows_t(cudaStream_t st, View<R> rhs, const long long* perm) {
+  Kind<R, CX>::permute_rows(st, rhs, perm);
+}
+template void permute_rows_t<double, false>(cudaStream_t, View<double>, const long long*);
+template void permute_rows_t<float, false>(cudaStream_t, View<float>, const long long*);
+template void permute_rows_t<double, true>(cudaStream_t, View<double>, const long long*);
+template void permute_rows_t<float, true>(cudaStream_t, View<float>, const long long*);
+
 }  // namespace fb

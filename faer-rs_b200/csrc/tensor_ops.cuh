@@ -114,6 +114,15 @@ void qr_reconstruct_t(cudaStream_t st, View<R> out, View<const R> Q_basis, View<
 template <class R, bool CX>
 void qr_inverse_t(cudaStream_t st, View<R> out, View<const R> Q_basis, View<const R> Q_coeff, View<const R> Rm);
 
+// rhs[i, :] <- rhs[perm[i], :] for every scalar kind (perm: HOST int64 of rhs.nrows entries; the row gather of the LU /
+// QR reconstructions); a column permutation is this on the transposed view
+template <class R, bool CX>
+void permute_rows_t(cudaStream_t st, View<R> rhs, const long long* perm);
+// cplx.cu: T(strict upper) <- V^H V for complex reflectors (upgrade_householder_factor with prev_block_size 1; views in COMPLEX
+// element units on an R* base), the twin of householder_build_t
+template <class R>
+void householder_build_t_cx(cudaStream_t st, View<const R> V, View<R> Tf);
+
 // dst(triangle) <- src(triangle)^-1 (triangular_inverse.rs), every scalar kind; only the triangle is written (not the diagonal if unit)
 template <class R, bool CX>
 void inverse_triangular_t(cudaStream_t st, View<R> dst, View<const R> src, bool lower, bool unit);

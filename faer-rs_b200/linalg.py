@@ -771,3 +771,66 @@ def piv_llt_inverse(out, L, perm, perm_inv, par=None) -> None:
     getattr(capi.load(), f"libfaer_v0_23_piv_llt_inverse_{_perm_width(perm)}_{suf}")(
         capi.mat_mut(out), capi.mat_ref(L), capi.slice_mut(perm), capi.slice_mut(perm_inv), par or capi.par_default(),
         capi.MemAlloc(None, 0))
+
+
+# ---- column-pivoted QR (qr::col_pivoting) ----------------------------------------------------------
+@dataclass
+class ColPivQrInfo:
+    transposition_count: int
+
+
+def colpiv_qr_params_default():
+    return capi.load().libfaer_v0_23_ColPivQrParams_f64()
+
+
+def colpiv_qr_in_place(A, Q_coeff, perm, perm_inv, par=None, params=None) -> ColPivQrInfo:
+    """qr::col_pivoting::factor::qr_in_place (col_pivoting/factor.rs:345-388): A P = Q R in place. Q_coeff: block_size x
+    min(m, n) (T blocks as qr_in_place); `perm`/`perm_inv`: uint32/uint64 arrays (numpy) or int32/int64 CUDA tensors of length
+    n, (A P)[:, j] = A[:, perm[j]]. f64, f32, c64 or c32."""
+    lib = capi.load()
+    suf = _same_suffix(A, Q_coeff)
+    params = params or getattr(lib, f"libfaer_v0_23_ColPivQrParams_{suf}")()
+    st = getattr(lib, f"libfaer_v0_23_colpiv_qr_factor_in_place_{_perm_width(perm)}_{suf}")(
+        capi.mat_mut(A), capi.mat_mut(Q_coeff), capi.slice_mut(perm), capi.slice_mut(perm_inv), par or capi.par_default(),
+        capi.MemAlloc(None, 0), params)
+    if st.tag != 0:
+        raise RuntimeError("ColPivQrStatus::Unknown")
+    return ColPivQrInfo(int(st.ok.transposition_count))
+
+
+def _colpiv_solve(name, Q_basis, Q_coeff, R, perm, perm_inv, rhs, conj, par):
+    suf = _same_suffix(Q_basis, Q_coeff, R, rhs)
+    getattr(capi.load(), f"libfaer_v0_23_colpiv_qr_{name}_in_place_{_perm_width(perm)}_{suf}")(
+        capi.mat_ref(Q_basis), capi.mat_ref(Q_coeff), capi.mat_ref(R), conj, capi.slice_mut(perm), capi.slice_mut(perm_inv),
+        capi.mat_mut(rhs), par or capi.par_default(), capi.MemAlloc(None, 0))
+
+
+def colpiv_qr_solve_in_place(Q_basis, Q_coeff, R, perm, perm_inv, rhs, conj: int = CONJ_NO, par=None) -> None:
+    """col_pivoting/solve.rs:107-131: rhs <- A^-1 rhs (conj(A)^-1 rhs with CONJ_YES), square A."""
+    _colpiv_solve("solve", Q_basis, Q_coeff, R, perm, perm_inv, rhs, conj, par)
+
+
+def colpiv_qr_solve_transpose_in_place(Q_basis, Q_coeff, R, perm, perm_inv, rhs, conj: int = CONJ_NO, par=None) -> None:
+    """col_pivoting/solve.rs:158-184: rhs <- A^-T rhs (A^-H with CONJ_YES), square A."""
+    _colpiv_solve("solve_transpose", Q_basis, Q_coeff, R, perm, perm_inv, rhs, conj, par)
+
+
+def colpiv_qr_solve_lstsq_in_place(Q_basis, Q_coeff, R, perm, perm_inv, rhs, conj: int = CONJ_NO, par=None) -> None:
+    """col_pivoting/solve.rs:52-80: least-squares solution (m >= n) left in rhs[:ncols, :]."""
+    _colpiv_solve("solve_lstsq", Q_basis, Q_coeff, R, perm, perm_inv, rhs, conj, par)
+
+
+def colpiv_qr_reconstruct(out, Q_basis, Q_coeff, R, perm, perm_inv, par=None) -> None:
+    """col_pivoting/reconstruct.rs:16-45: out <- Q R P^T."""
+    suf = _same_suffix(out, Q_basis, Q_coeff, R)
+    getattr(capi.load(), f"libfaer_v0_23_colpiv_qr_reconstruct_{_perm_width(perm)}_{suf}")(
+        capi.mat_mut(out), capi.mat_ref(Q_basis), capi.mat_ref(Q_coeff), capi.mat_ref(R), capi.slice_mut(perm),
+        capi.slice_mut(perm_inv), par or capi.par_default(), capi.MemAlloc(None, 0))
+
+
+def colpiv_qr_inverse(out, Q_basis, Q_coeff, R, perm, perm_inv, par=None) -> None:
+    """col_pivoting/inverse.rs:16-50: out <- A^-1 = P R^-1 Q^H, square A."""
+    suf = _same_suffix(out, Q_basis, Q_coeff, R)
+    getattr(capi.load(), f"libfaer_v0_23_colpiv_qr_inverse_{_perm_width(perm)}_{suf}")(
+        capi.mat_mut(out), capi.mat_ref(Q_basis), capi.mat_ref(Q_coeff), capi.mat_ref(R), capi.slice_mut(perm),
+        capi.slice_mut(perm_inv), par or capi.par_default(), capi.MemAlloc(None, 0))

@@ -6,10 +6,11 @@ Reference: faer/src/linalg/solvers.rs
     split_LU                                    955-980   (packed factors -> unit-lower L and upper U, both owned)
     PartialPivLu::new / L / U / P               981-1034
     Qr::new / Q_basis / Q_coeff / R / thin_R / compute_Q / compute_thin_Q   1106-1205
+    ColPivQr::new / Q_basis / Q_coeff / R / thin_R / P / compute_Q / compute_thin_Q   1206-1260
     Solve / SolveLstsq extension traits         93-282, 639-690  (solve, solve_conjugate, solve_transpose, solve_adjoint and
                                                                    the rsolve_* family through the transposed system)
-    SolveCore impls                             1861-1905 (Llt), 2147-2196 (PartialPivLu), 2339-2418 (Qr)
-    DenseSolveCore::reconstruct                 1917-1936 (Llt), 2198-2217 (PartialPivLu), 2420-2440 (Qr)
+    SolveCore impls                             1861-1905 (Llt), 2147-2196 (PartialPivLu), 2339-2418 (Qr), 2462-2530 (ColPivQr)
+    DenseSolveCore::reconstruct / inverse       1917-1936 (Llt), 2198-2217 (PartialPivLu), 2420-2440 (Qr), 2532-2560 (ColPivQr)
 and faer/src/mat/mat_ops.rs:869-897 (`Mul` for matrices -> `mul`).
 
 Every flop runs in libfaer_b200.so through `linalg.py`; this module only owns buffers, splits the packed factors and
@@ -487,6 +488,62 @@ class Qr(_Solve):
         return out
 
 
+class ColPivQr(Qr):
+    """A P = Q R, column-pivoted Householder QR (solvers.rs:738, 1206-1260, 2462-2560). `P()` returns (perm_fwd, perm_bwd):
+    (A P)[:, j] = A[:, perm_fwd[j]]. Q is kept as for `Qr`; solves, reconstruct and inverse go through the library's
+    `colpiv_qr_*` entry points, which apply the permutation."""
+
+    def __init__(self, Q_basis, Q_coeff, R, fwd, bwd, m, n):
+        super().__init__(Q_basis, Q_coeff, R, m, n)
+        self._fwd, self._bwd = fwd, bwd
+
+    @classmethod
+    def new(cls, A) -> "ColPivQr":
+        assert A.ndim == 2
+        QR = _owned(A)
+        m, n = QR.shape
+        size = min(m, n)
+        bs = la.qr_recommended_block_size(m, n)
+        Q_coeff = _zeros(QR, bs, size)
+        if _t(QR):
+            import torch
+            fwd = torch.zeros(n, dtype=torch.int64, device=QR.device)
+            bwd = torch.zeros(n, dtype=torch.int64, device=QR.device)
+        else:
+            fwd = np.zeros(n, dtype=np.uint64)
+            bwd = np.zeros(n, dtype=np.uint64)
+        la.colpiv_qr_in_place(QR, Q_coeff, fwd, bwd)
+        Q_basis, R = split_LU(QR)
+        return cls(Q_basis, Q_coeff, R, fwd, bwd, m, n)
+
+    def P(self):
+        return self._fwd, self._bwd
+
+    def _solve_core(self, rhs, conj: int) -> None:
+        la.colpiv_qr_solve_in_place(self._Qb, self._Qc, self._R, self._fwd, self._bwd, rhs, conj)
+
+    def _solve_transpose_core(self, rhs, conj: int) -> None:
+        la.colpiv_qr_solve_transpose_in_place(self._Qb, self._Qc, self._R, self._fwd, self._bwd, rhs, conj)
+
+    def _lstsq(self, rhs, conj: int) -> None:
+        r = _as_2d(rhs)
+        assert self._m == r.shape[0] and self._m >= self._n
+        la.colpiv_qr_solve_lstsq_in_place(self._Qb, self._Qc, self._R, self._fwd, self._bwd, r, conj)
+
+    def reconstruct(self):
+        """col_pivoting/reconstruct.rs: Q R P^T."""
+        out = _zeros(self._R, self._m, self._n)
+        la.colpiv_qr_reconstruct(out, self._Qb, self._Qc, self.thin_R(), self._fwd, self._bwd)
+        return out
+
+    def inverse(self):
+        """col_pivoting/inverse.rs: P R^-1 Q^H (square A)."""
+        assert self._m == self._n
+        out = _zeros(self._R, self._n, self._n)
+        la.colpiv_qr_inverse(out, self._Qb, self._Qc, self._R, self._fwd, self._bwd)
+        return out
+
+
 class Svd:
     """`Svd<T>` (solvers.rs:1324-1400): `new` = full U and V, `new_thin` = the first min(nrows, ncols) columns of each;
     A = U diag(S) V^H, S non-increasing. Accessors U(), V(), S() as in the reference; pseudoinverse() = V S^+ U^H
@@ -598,6 +655,10 @@ def partial_piv_lu(A) -> PartialPivLu:
 
 def qr(A) -> Qr:
     return Qr.new(A)
+
+
+def colpiv_qr(A) -> ColPivQr:
+    return ColPivQr.new(A)
 
 
 def singular_values(A):

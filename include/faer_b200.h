@@ -713,5 +713,7 @@ void libfaer_v0_23_partial_piv_lu_solve_transpose_in_place_u64_c32(struct FaerV0
 
 /* pivoted Cholesky (piv_llt_*): declared in its own header */
 #include "faer_b200_piv_llt.h"
+/* column-pivoted QR (colpiv_qr_*): declared in its own header */
+#include "faer_b200_colpiv_qr.h"
 
 #endif /* LIBFAER_V0_24 */
