@@ -173,6 +173,25 @@ class ColPivQrStatus(C.Structure):
     _fields_ = [("tag", C.c_int), ("body", _ColPivQrBody)]
 
 
+class FullPivLuParams(C.Structure):
+    """faer.h:128-130."""
+    _fields_ = [("par_threshold", C.c_size_t)]
+
+
+class _FullPivLuOkBody(C.Structure):
+    _fields_ = [("transposition_count", C.c_size_t)]
+
+
+class _FullPivLuBody(C.Union):
+    _fields_ = [("ok", _FullPivLuOkBody)]
+
+
+class FullPivLuStatus(C.Structure):
+    """tag: 0 Ok{transposition_count}, 1 Unknown (faer.h:287-301); 16 bytes, body at 8."""
+    _anonymous_ = ("body",)
+    _fields_ = [("tag", C.c_int), ("body", _FullPivLuBody)]
+
+
 ACCUM_REPLACE, ACCUM_ADD = 0, 1
 CONJ_NO, CONJ_YES = 0, 1
 PAR_SEQ, PAR_RAYON = 0, 1
@@ -468,6 +487,34 @@ def load() -> C.CDLL:
             for name in ("reconstruct", "inverse"):
                 f = getattr(lib, f"{pre}{name}_{it}_{suf}")
                 f.argtypes = [MatMut, MatRef, MatRef, MatRef, SliceMut, SliceMut, P, MemAlloc]
+                f.restype = None
+    for suf in ("f64", "f32", "c64", "c32"):
+        getattr(lib, f"libfaer_v0_23_FullPivLuParams_{suf}").argtypes = []
+        getattr(lib, f"libfaer_v0_23_FullPivLuParams_{suf}").restype = FullPivLuParams
+        for it in ("u32", "u64"):
+            pre = "libfaer_v0_23_full_piv_lu_"
+            f = getattr(lib, f"{pre}factor_in_place_scratch_{it}_{suf}")
+            f.argtypes = [C.c_size_t, C.c_size_t, P, FullPivLuParams]
+            f.restype = Layout
+            f = getattr(lib, f"{pre}factor_in_place_{it}_{suf}")
+            f.argtypes = [MatMut, SliceMut, SliceMut, SliceMut, SliceMut, P, MemAlloc, FullPivLuParams]
+            f.restype = FullPivLuStatus
+            for name in ("solve", "solve_transpose"):
+                f = getattr(lib, f"{pre}{name}_in_place_scratch_{it}_{suf}")
+                f.argtypes = [C.c_size_t, C.c_size_t, P]
+                f.restype = Layout
+                f = getattr(lib, f"{pre}{name}_in_place_{it}_{suf}")
+                f.argtypes = [MatRef, MatRef, C.c_int, SliceMut, SliceMut, SliceMut, SliceMut, MatMut, P, MemAlloc]
+                f.restype = None
+            f = getattr(lib, f"{pre}reconstruct_scratch_{it}_{suf}")
+            f.argtypes = [C.c_size_t, C.c_size_t, P]
+            f.restype = Layout
+            f = getattr(lib, f"{pre}inverse_scratch_{it}_{suf}")
+            f.argtypes = [C.c_size_t, P]
+            f.restype = Layout
+            for name in ("reconstruct", "inverse"):
+                f = getattr(lib, f"{pre}{name}_{it}_{suf}")
+                f.argtypes = [MatMut, MatRef, MatRef, SliceMut, SliceMut, SliceMut, SliceMut, P, MemAlloc]
                 f.restype = None
     lib.faer_b200_version.argtypes = []
     lib.faer_b200_version.restype = C.c_char_p

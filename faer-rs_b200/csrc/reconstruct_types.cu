@@ -75,6 +75,19 @@ struct RtScatterBack {
   }
 };
 
+// out[i, j] = src[p[i], q[j]]
+template <class R, int W>
+struct RtGather2d {
+  R* out; i64 o_rs, o_cs; const R* src; i64 s_rs, s_cs, m, n; const long long* p; const long long* q;
+  RT_HD void operator()(i64 i, i64 j) const {
+    if (i >= m || j >= n) return;
+    const R* s = src + W * (p[i] * s_rs + q[j] * s_cs);
+    R* d = out + W * (i * o_rs + j * o_cs);
+    d[0] = s[0];
+    if (W == 2) d[W - 1] = s[W - 1];
+  }
+};
+
 // dst(i, j) = src(i, j) on the triangle `lower` selects — diagonal included unless `unit` — and nothing elsewhere
 template <class R, int W>
 struct RtCopyTriangle {
@@ -284,5 +297,23 @@ template void permute_rows_t<double, false>(cudaStream_t, View<double>, const lo
 template void permute_rows_t<float, false>(cudaStream_t, View<float>, const long long*);
 template void permute_rows_t<double, true>(cudaStream_t, View<double>, const long long*);
 template void permute_rows_t<float, true>(cudaStream_t, View<float>, const long long*);
+
+template <class R, bool CX>
+void gather_2d_t(cudaStream_t st, View<R> out, View<const R> src, const long long* p, const long long* q) {
+  constexpr int W = CX ? 2 : 1;
+  const i64 m = out.nrows, n = out.ncols;
+  if (m == 0 || n == 0) return;
+  long long* d_p = (long long*)ws_alloc((size_t)(m + n) * 8);
+  FB_CUDA_CHECK(cudaMemcpyAsync(d_p, p, (size_t)m * 8, cudaMemcpyHostToDevice, st));
+  FB_CUDA_CHECK(cudaMemcpyAsync(d_p + m, q, (size_t)n * 8, cudaMemcpyHostToDevice, st));
+  DevRun run{st};
+  run(RtGather2d<R, W>{out.ptr, out.rs, out.cs, src.ptr, src.rs, src.cs, m, n, d_p, d_p + m}, m, n);
+  FB_CUDA_CHECK(cudaStreamSynchronize(st));  // p / q (host, pageable) and the pool buffer are released by the caller / below
+  ws_free(d_p);
+}
+template void gather_2d_t<double, false>(cudaStream_t, View<double>, View<const double>, const long long*, const long long*);
+template void gather_2d_t<float, false>(cudaStream_t, View<float>, View<const float>, const long long*, const long long*);
+template void gather_2d_t<double, true>(cudaStream_t, View<double>, View<const double>, const long long*, const long long*);
+template void gather_2d_t<float, true>(cudaStream_t, View<float>, View<const float>, const long long*, const long long*);
 
 }  // namespace fb

@@ -118,6 +118,10 @@ void qr_inverse_t(cudaStream_t st, View<R> out, View<const R> Q_basis, View<cons
 // QR reconstructions); a column permutation is this on the transposed view
 template <class R, bool CX>
 void permute_rows_t(cudaStream_t st, View<R> rhs, const long long* perm);
+// out[i, j] <- src[p[i], q[j]] for every scalar kind (p, q: HOST int64 of out.nrows / out.ncols entries; out and src must not
+// overlap); the permuted 2-D gather of the full-pivoting LU reconstruct / inverse
+template <class R, bool CX>
+void gather_2d_t(cudaStream_t st, View<R> out, View<const R> src, const long long* p, const long long* q);
 // cplx.cu: T(strict upper) <- V^H V for complex reflectors (upgrade_householder_factor with prev_block_size 1; views in COMPLEX
 // element units on an R* base), the twin of householder_build_t
 template <class R>

@@ -834,3 +834,68 @@ def colpiv_qr_inverse(out, Q_basis, Q_coeff, R, perm, perm_inv, par=None) -> Non
     getattr(capi.load(), f"libfaer_v0_23_colpiv_qr_inverse_{_perm_width(perm)}_{suf}")(
         capi.mat_mut(out), capi.mat_ref(Q_basis), capi.mat_ref(Q_coeff), capi.mat_ref(R), capi.slice_mut(perm),
         capi.slice_mut(perm_inv), par or capi.par_default(), capi.MemAlloc(None, 0))
+
+
+# ---- full-pivoting LU (lu::full_pivoting) ----------------------------------------------------------
+@dataclass
+class FullPivLuInfo:
+    transposition_count: int
+
+
+def full_piv_lu_params_default():
+    return capi.load().libfaer_v0_23_FullPivLuParams_f64()
+
+
+def full_piv_lu_in_place(A, row_perm, row_perm_inv, col_perm, col_perm_inv, par=None, params=None) -> FullPivLuInfo:
+    """lu::full_pivoting::factor::lu_in_place (full_pivoting/factor.rs:466-538): P A Q = L U in place (L unit-lower below the
+    diagonal, U on and above it). `row_perm`/`row_perm_inv` (length m) and `col_perm`/`col_perm_inv` (length n): uint32/uint64
+    arrays (numpy) or int32/int64 CUDA tensors of one width; (P A Q)[i, j] = A[row_perm[i], col_perm[j]]. f64, f32, c64 or c32."""
+    lib = capi.load()
+    suf = _suf_lu(A)
+    params = params or getattr(lib, f"libfaer_v0_23_FullPivLuParams_{suf}")()
+    par = par or capi.par_default()
+    it = _perm_width(row_perm)
+    assert _perm_width(col_perm) == it
+    m, n = A.shape
+    lay = getattr(lib, f"libfaer_v0_23_full_piv_lu_factor_in_place_scratch_{it}_{suf}")(m, n, par, params)
+    scratch = np.empty(lay.len_bytes + lay.align_bytes, dtype=np.uint8)
+    st = getattr(lib, f"libfaer_v0_23_full_piv_lu_factor_in_place_{it}_{suf}")(
+        capi.mat_mut(A), capi.slice_mut(row_perm), capi.slice_mut(row_perm_inv), capi.slice_mut(col_perm),
+        capi.slice_mut(col_perm_inv), par, capi.MemAlloc(scratch.ctypes.data, scratch.size), params)
+    if st.tag != 0:
+        raise RuntimeError("FullPivLuStatus::Unknown")
+    return FullPivLuInfo(int(st.ok.transposition_count))
+
+
+def _full_piv_lu_solve(name, L, U, row_perm, row_perm_inv, col_perm, col_perm_inv, rhs, conj, par):
+    suf = _same_suffix(L, U, rhs)
+    getattr(capi.load(), f"libfaer_v0_23_full_piv_lu_{name}_in_place_{_perm_width(row_perm)}_{suf}")(
+        capi.mat_ref(L), capi.mat_ref(U), conj, capi.slice_mut(row_perm), capi.slice_mut(row_perm_inv), capi.slice_mut(col_perm),
+        capi.slice_mut(col_perm_inv), capi.mat_mut(rhs), par or capi.par_default(), capi.MemAlloc(None, 0))
+
+
+def full_piv_lu_solve_in_place(L, U, row_perm, row_perm_inv, col_perm, col_perm_inv, rhs, conj: int = CONJ_NO, par=None) -> None:
+    """full_pivoting/solve.rs:21-56: rhs <- A^-1 rhs (conj(A)^-1 rhs with CONJ_YES), square A. L and U may be the packed factor."""
+    _full_piv_lu_solve("solve", L, U, row_perm, row_perm_inv, col_perm, col_perm_inv, rhs, conj, par)
+
+
+def full_piv_lu_solve_transpose_in_place(L, U, row_perm, row_perm_inv, col_perm, col_perm_inv, rhs, conj: int = CONJ_NO,
+                                         par=None) -> None:
+    """full_pivoting/solve.rs:58-93: rhs <- A^-T rhs (A^-H with CONJ_YES), square A."""
+    _full_piv_lu_solve("solve_transpose", L, U, row_perm, row_perm_inv, col_perm, col_perm_inv, rhs, conj, par)
+
+
+def full_piv_lu_reconstruct(out, L, U, row_perm, row_perm_inv, col_perm, col_perm_inv, par=None) -> None:
+    """full_pivoting/reconstruct.rs:13-82: out (m x n) <- P^-1 L U Q^-1."""
+    suf = _same_suffix(out, L, U)
+    getattr(capi.load(), f"libfaer_v0_23_full_piv_lu_reconstruct_{_perm_width(row_perm)}_{suf}")(
+        capi.mat_mut(out), capi.mat_ref(L), capi.mat_ref(U), capi.slice_mut(row_perm), capi.slice_mut(row_perm_inv),
+        capi.slice_mut(col_perm), capi.slice_mut(col_perm_inv), par or capi.par_default(), capi.MemAlloc(None, 0))
+
+
+def full_piv_lu_inverse(out, L, U, row_perm, row_perm_inv, col_perm, col_perm_inv, par=None) -> None:
+    """full_pivoting/inverse.rs:12-63: out <- A^-1 = Q U^-1 L^-1 P, square A."""
+    suf = _same_suffix(out, L, U)
+    getattr(capi.load(), f"libfaer_v0_23_full_piv_lu_inverse_{_perm_width(row_perm)}_{suf}")(
+        capi.mat_mut(out), capi.mat_ref(L), capi.mat_ref(U), capi.slice_mut(row_perm), capi.slice_mut(row_perm_inv),
+        capi.slice_mut(col_perm), capi.slice_mut(col_perm_inv), par or capi.par_default(), capi.MemAlloc(None, 0))

@@ -400,6 +400,72 @@ class PartialPivLu(_Solve):
         return out
 
 
+class FullPivLu(_Solve):
+    """P A Q = L U with full pivoting (solvers.rs:1036-1105; SolveCore 2241-2292, DenseSolveCore 2294-2330). `P()` / `Q()`
+    return (perm_fwd, perm_bwd): (P A Q)[i, j] = A[P_fwd[i], Q_fwd[j]]."""
+
+    def __init__(self, L, U, row, col, m, n):
+        self._L, self._U, self._row, self._col, self._m, self._n = L, U, row, col, m, n
+
+    @classmethod
+    def new(cls, A) -> "FullPivLu":
+        assert A.ndim == 2
+        LU = _owned(A)
+        m, n = LU.shape
+
+        def perm(k):
+            if _t(LU):
+                import torch
+                return torch.zeros(k, dtype=torch.int64, device=LU.device)
+            return np.zeros(k, dtype=np.uint64)
+
+        row = (perm(m), perm(m))
+        col = (perm(n), perm(n))
+        la.full_piv_lu_in_place(LU, row[0], row[1], col[0], col[1])
+        L, U = split_LU(LU)
+        return cls(L, U, row, col, m, n)
+
+    def L(self):
+        return self._L
+
+    def U(self):
+        return self._U
+
+    def P(self):
+        return self._row
+
+    def Q(self):
+        return self._col
+
+    def nrows(self) -> int:
+        return self._m
+
+    def ncols(self) -> int:
+        return self._n
+
+    def _like(self):
+        return self._L
+
+    def _solve_core(self, rhs, conj: int) -> None:
+        la.full_piv_lu_solve_in_place(self._L, self._U, *self._row, *self._col, rhs, conj)
+
+    def _solve_transpose_core(self, rhs, conj: int) -> None:
+        la.full_piv_lu_solve_transpose_in_place(self._L, self._U, *self._row, *self._col, rhs, conj)
+
+    def reconstruct(self):
+        """full_pivoting/reconstruct.rs:13-82: A from the factors."""
+        out = _zeros(self._L, self._m, self._n)
+        la.full_piv_lu_reconstruct(out, self._L, self._U, *self._row, *self._col)
+        return out
+
+    def inverse(self):
+        """full_pivoting/inverse.rs:12-63."""
+        assert self._m == self._n
+        out = _zeros(self._L, self._m, self._m)
+        la.full_piv_lu_inverse(out, self._L, self._U, *self._row, *self._col)
+        return out
+
+
 class Qr(_Solve):
     """A = Q R, Householder QR without pivoting (solvers.rs:1106-1205). Q is kept as the Householder basis (unit-lower
     trapezoid) and the block coefficients; `compute_Q` / `compute_thin_Q` form it."""
@@ -651,6 +717,10 @@ def ldlt(A, side: int = Side.Lower) -> Ldlt:
 
 def partial_piv_lu(A) -> PartialPivLu:
     return PartialPivLu.new(A)
+
+
+def full_piv_lu(A) -> FullPivLu:
+    return FullPivLu.new(A)
 
 
 def qr(A) -> Qr:
