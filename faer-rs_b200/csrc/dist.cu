@@ -295,16 +295,25 @@ static LltHostPipe* g_llt_pipe = nullptr;
 // the tail (remaining order <= FAER_B200_LLT_TAIL, default 6144) the panel chain does — potf2 + the 128-wide TRSM / SYRK
 // inside a 256-block + the panel solve's leaves; 128-wide blocks have no inner recursion and half the leaves — so the
 // blocks narrow to 128 there. P > 1 keeps uniform blocks (ownership is b % P).
-static std::vector<i64> llt_block_bounds(i64 n, i64 nb, bool uniform) {
-  static i64 tail = -1;
+// `wide_head` (the device-resident driver at its default width): while the remaining order exceeds FAER_B200_LLT_HEAD
+// (default 8192) the blocks are 512 wide: contracting k = 512 per update halves how often the SYRK pays its per-tile
+// fixed cost and how often the trailing matrix crosses HBM, while a step's trailing update (~ m^2) still hides the
+// longer 512-wide panel chain. At n = 16384 every boundary from 6144 to 10240 measured the same within noise
+// (profiles/r08_bench_parent_vs_branch.json).
+static std::vector<i64> llt_block_bounds(i64 n, i64 nb, bool uniform, bool wide_head = false) {
+  static i64 tail = -1, head = -1;
   if (tail < 0) {
     const char* e = getenv("FAER_B200_LLT_TAIL");
     tail = e ? atoll(e) : 6144;
+    const char* h = getenv("FAER_B200_LLT_HEAD");
+    head = h ? atoll(h) : 8192;
   }
   std::vector<i64> b0;
   for (i64 c = 0; c < n;) {
     b0.push_back(c);
-    const i64 w = (!uniform && nb > 128 && n - c <= tail) ? 128 : nb;
+    i64 w = nb;
+    if (!uniform && nb > 128 && n - c <= tail) w = 128;
+    else if (!uniform && wide_head && n - c > head) w = 512;
     c += std::min<i64>(w, n - c);
   }
   b0.push_back(n);
@@ -324,7 +333,7 @@ i64 lookahead_block() {
   static i64 v = -1;
   if (v < 0) {
     const char* e = getenv("FAER_B200_NB");
-    v = e ? atoll(e) : 0;  // 0 = caller's default (LLT 1024; LU 512 up to n = 20000, then 1024)
+    v = e ? atoll(e) : 0;  // 0 = caller's default (LLT 512 / 256 / 128, see llt_block_bounds; LU 512 up to n = 20000, then 1024)
     if (v < 0 || (v & 1)) v = 0;
   }
   return v;
@@ -483,8 +492,10 @@ static LltResult llt_local_partitioned_f64(double* A, i64 ld, i64 n, i64 nb, dou
 // -----------------------------------------------------------------------------------------------------------------
 LltResult dist_llt_f64(double* A_local, i64 ld, i64 n, i64 nb, double reg_delta, double reg_eps, int lookahead) {
   FB_ENTRY();
-  // `lookahead` bit 0: two-stream look-ahead; bit 1: purely local run (ignore the communicator even if one exists)
+  // `lookahead` bit 0: two-stream look-ahead; bit 1: purely local run (ignore the communicator even if one exists);
+  // bit 2: 512-wide leading blocks (llt_block_bounds' wide_head; single GPU, device-resident matrix, look-ahead only)
   const bool local_only = (lookahead & 2) != 0;
+  const bool wide_head = (lookahead & 4) != 0;
   lookahead &= 1;
   const int P = (g_comm && !local_only) ? g_nranks : 1, me = (g_comm && !local_only) ? g_rank : 0;
   LltResult res{true, 0, 0};
@@ -507,13 +518,15 @@ LltResult dist_llt_f64(double* A_local, i64 ld, i64 n, i64 nb, double reg_delta,
   FB_CUDA_CHECK(cudaStreamWaitEvent(sp, ev_start, 0));
   if (two_streams) FB_CUDA_CHECK(cudaStreamWaitEvent(sm, ev_start, 0));
 
-  const std::vector<i64> b0 = llt_block_bounds(n, nb, /*uniform*/ P > 1 || !lookahead);
+  const std::vector<i64> b0 = llt_block_bounds(n, nb, /*uniform*/ P > 1 || !lookahead, wide_head && P == 1 && !pipe);
   const i64 nblk = (i64)b0.size() - 1;
   auto col_off = [&](i64 b) { return P == 1 ? b0[(size_t)b] : local_off(b, nb, P) ; };  // local column of block b (owned)
+  i64 wmax = 0;
+  for (i64 k = 0; k < nblk; ++k) wmax = std::max(wmax, b0[(size_t)k + 1] - b0[(size_t)k]);
   // two panel buffers (double buffering for look-ahead)
   double* W[2];
-  W[0] = (double*)ws_alloc((size_t)n * nb * 8);
-  W[1] = (double*)ws_alloc((size_t)n * nb * 8);
+  W[0] = (double*)ws_alloc((size_t)n * wmax * 8);
+  W[1] = (double*)ws_alloc((size_t)n * wmax * 8);
   long long* d_info = (long long*)ws_alloc(4 * sizeof(long long));
   long long h_info[2] = {-1, 0};
   FB_CUDA_CHECK(cudaMemcpyAsync(d_info, h_info, sizeof(h_info), cudaMemcpyHostToDevice, sp));

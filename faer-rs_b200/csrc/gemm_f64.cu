@@ -488,15 +488,16 @@ void gemm_f64(cudaStream_t stream, VD dst, int dst_struct, int accum, VCD lhs, i
   }
   // large rectangular-operand products: the TMA-fed warp-specialised kernel (gemm_f64_ws.cuh)
   if (ws_mode() != 0 && !split_ws) {
-    // Heuristic. Triangular destinations with k <= 512 and >= 3 waves of 128 x 128 tiles (one CTA per SM) take the wide
-    // configuration: the SYRK trailing updates of LLT. Other products take the narrow one when their 128 x 64 tiles fill
+    // Heuristic. Triangular destinations with k <= 1024 and >= 3 waves of 128 x 128 tiles (one CTA per SM) take the wide
+    // configuration: the SYRK trailing updates of LLT (at n = 16128 it beat the narrow one at k = 768 and 1024 too,
+    // profiles/r08_gemm_f64_shapes.log). Other products take the narrow one when their 128 x 64 tiles fill
     // >= 3 waves of two CTAs per SM and their contraction is deep enough to amortise a tile's epilogue (k >= 512: at
     // k = 256 the cp.async kernel is faster even on a full 16384 x 16384 update, profiles/r03_gemm_f64_shapes.log); the
     // cp.async kernel (64 x 64 tiles, three CTAs per SM) keeps short contractions and products with few tiles.
     // gemm_ws = 2 forces the narrow configuration, 3 the wide one.
     const int sms = stream_sms(stream);
     const bool wide = ws_mode() == 3 ||
-                      (ws_mode() == 1 && dst_struct != RECT && p.k <= 512 &&
+                      (ws_mode() == 1 && dst_struct != RECT && p.k <= 1024 &&
                        ws64::ws_tiles(p.m, p.n, dst_struct, ws64::Shape<true>::BN) >= 3ll * sms);
     long long tiles_narrow = (long long)((p.m + ws64::BM - 1) / ws64::BM) * ((p.n + ws64::Shape<false>::BN - 1) / ws64::Shape<false>::BN);
     if (dst_struct != RECT) tiles_narrow = tiles_narrow / 2 + 1;

@@ -53,8 +53,11 @@ constexpr int A_BYTES = BM * BK * 8;               // 16 KB
 //     32 KB and a 128 KB destination buffer, one CTA per SM. Per DMMA it reads half the operand bytes of the 64 x 64
 //     cp.async tile (16 instead of 32 B per clock and SM at the full DMMA rate). Tiles that lie wholly inside the kept
 //     part of dst are combined in shared memory: the producer TMA-loads the old dst tile while the tile's main loop runs
-//     (Add mode), the consumers write alpha * acc [+ old] into the buffer and one thread TMA-stores it, so the next tile's
-//     main loop starts while the store drains. Tiles that straddle the diagonal of a triangular dst keep the masked
+//     (Add mode), the consumers write alpha * acc [+ old] into the buffer, signal `dst_ready` and go straight into the
+//     next tile's main loop; a storer warp of the producer warpgroup TMA-stores the buffer and frees it once the store
+//     has read it. With one CTA per SM nothing else covers a consumer stall, so no consumer waits for a store or for the
+//     other consumers at a tile's end. (The tensor form of cp.reduce.async.bulk has no f64 add, so Add mode keeps the
+//     TMA load of the old tile.) Tiles that straddle the diagonal of a triangular dst keep the masked
 //     register epilogue (the untouched triangle must not be written, not even with its own values).
 template <bool WIDE>
 struct Shape {
@@ -211,6 +214,7 @@ gemm_f64_ws_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
   uint64_t* empty = full + STAGES;
   uint64_t* dst_full = empty + STAGES;   // wide: old dst values landed (Add) / buffer free to overwrite (Replace)
   uint64_t* dst_free = dst_full + 1;     // wide: the previous TMA store has read the buffer
+  uint64_t* dst_ready = dst_free + 1;    // wide: every consumer warp has written its part of the buffer
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
@@ -220,6 +224,7 @@ gemm_f64_ws_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
     }
     mbar_init(dst_full, 1);
     mbar_init(dst_free, 1);
+    mbar_init(dst_ready, CONSUMERS);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -280,6 +285,27 @@ gemm_f64_ws_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
             ++ds;
           }
         }
+      }
+    }
+    if constexpr (WIDE) {
+      // storer (warp 1): TMA-stores each staged tile once the consumers have filled the buffer, and frees the buffer
+      // when the store has read it, so that the consumers go from one tile's epilogue straight into the next main loop
+      if (warp == 1 && lane == 0) {
+        uint32_t ds = 0;
+        for (int i = 0; i < p.tiles_per_cta; ++i) {
+          int tm, tn;
+          if (!walk.locate((int)blockIdx.x * p.tiles_per_cta + i, tm, tn)) break;
+          if (!staged(tm, tn)) continue;
+          mbar_wait(dst_ready, ds & 1u);
+          ++ds;
+#pragma unroll
+          for (int b = 0; b < BM / 16; ++b) tma_store_2d(&mapC, sdst + b * (16 * BN * 8), tm * BM + b * 16, tn * BN);
+          asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+          asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+          mbar_arrive(dst_free);
+        }
+        // the tile stores must have completed before the kernel ends
+        asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
       }
     }
     return;
@@ -388,7 +414,7 @@ gemm_f64_ws_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
     }
 
     if (staged(tm, tn)) {
-      // ---- wide epilogue through shared memory: buffer = alpha * acc [+ old], then one TMA store of the tile. Element
+      // ---- wide epilogue through shared memory: buffer = alpha * acc [+ old], then the storer warp's TMA store. Element
       // (r, c) of the tile sits in box r / 16 at line c, 16-byte chunk ((r & 15) / 2) ^ (c & 7): a half-warp's 8-byte
       // accesses (4 rows x 4 column pairs) hit 16 distinct banks ----
       mbar_wait(dst_full, dc & 1u);
@@ -409,14 +435,8 @@ gemm_f64_ws_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
       }
       // the generic-proxy writes above must be visible to the async proxy (the TMA store) before it reads the buffer
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      asm volatile("bar.sync 1, %0;" ::"n"(CONSUMERS * 32) : "memory");
-      if (cw == 0 && lane == 0) {
-#pragma unroll
-        for (int b = 0; b < BM / 16; ++b) tma_store_2d(&mapC, sdst + b * (16 * BN * 8), m0 + b * 16, n0);
-        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-        asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-        mbar_arrive(dst_free);
-      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(dst_ready);
       continue;
     }
 
@@ -470,8 +490,6 @@ gemm_f64_ws_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
       }
     }
   }
-  // the tile stores must have completed before the kernel ends
-  if (WIDE && cw == 0 && lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,

@@ -253,10 +253,11 @@ LltResult llt_cholesky_in_place_f64(cudaStream_t stream, VD A, double reg_delta,
   // Large column-major problems: right-looking block-column driver with two-stream look-ahead (dist.cu run on a
   // single rank): the panel chain (potf2 + solves of block column k+1) overlaps the trailing update of step k.
   if (A.rs == 1 && n >= lookahead_min_n()) {
-    // block width: with the trailing update of a step as ONE structured launch the short chain of narrow blocks keeps
-    // the panel chain short (FAER_B200_NB overrides)
-    const i64 nbl = lookahead_block() ? lookahead_block() : 256;
-    return dist_llt_f64(A.ptr, A.cs, n, nbl, reg_delta, reg_eps, /*lookahead | local*/ 3);
+    // block width: with the trailing update of a step as ONE structured launch, 512-wide blocks while the trailing matrix
+    // is large, then 256, then 128 in the tail keep the panel chain short (dist.cu: llt_block_bounds); FAER_B200_NB
+    // overrides the 512 / 256 tiers with one width
+    if (lookahead_block()) return dist_llt_f64(A.ptr, A.cs, n, lookahead_block(), reg_delta, reg_eps, /*lookahead | local*/ 3);
+    return dist_llt_f64(A.ptr, A.cs, n, 256, reg_delta, reg_eps, /*lookahead | local | wide head*/ 7);
   }
   return llt_recursive_in_place<double>(stream, A, reg_delta, reg_eps, params);
 }

@@ -124,8 +124,10 @@ def _bind(lib) -> None:
 
 
 # ---- distributed LLT ---------------------------------------------------------------------------------
-def cholesky_in_place(A_local, n: int, nb: int = 512, regularization=(0.0, 0.0), lookahead: bool = True):
+def cholesky_in_place(A_local, n: int, nb: int = 512, regularization=(0.0, 0.0), lookahead=True):
     """Distributed in-place LLT. `A_local`: torch CUDA tensor, column-major view (n x local_cols, stride (1, ld)).
+    `lookahead`: bool, or the driver's bit mask (1 = look-ahead, 2 = purely local run, 4 = 512-wide leading blocks on
+    one GPU, the schedule of the single-GPU entry point).
     Returns (fail_index or -1, regularisation count) reduced over the ranks of the default process group (if any)."""
     import torch
     lib = capi.load()
@@ -135,7 +137,8 @@ def cholesky_in_place(A_local, n: int, nb: int = 512, regularization=(0.0, 0.0),
     ld = A_local.stride(1) if A_local.shape[1] > 1 else max(n, 1)
     delta = C.c_double(float(regularization[0])); eps = C.c_double(float(regularization[1]))
     reg = capi.LltRegularization(C.cast(C.pointer(delta), C.c_void_p), C.cast(C.pointer(eps), C.c_void_p))
-    st = lib.faer_b200_dist_llt_factor_in_place_f64(A_local.data_ptr(), ld, n, nb, reg, 1 if lookahead else 0)
+    st = lib.faer_b200_dist_llt_factor_in_place_f64(A_local.data_ptr(), ld, n, nb, reg,
+                                                    int(lookahead) if not isinstance(lookahead, bool) else (1 if lookahead else 0))
     fail = int(st.value) if st.tag == 1 else -1
     cnt = int(st.value) if st.tag == 0 else 0
     try:

@@ -24,14 +24,18 @@ def best(f, reps=5):
 
 
 tag = f"stagger={os.environ.get('FAER_B200_WS_STAGGER', '1')}"
-# lower-triangular updates of the headline LLT (k = 256, and k = 128 in its last 6144 columns), and deeper ones
-for (n, k) in [(16128, 256), (12288, 256), (8192, 256), (4096, 256), (1024, 256), (6016, 128), (3072, 128), (16128, 512)]:
+# lower-triangular updates of the headline LLT (k = 512 / 256 / 128 by remaining order), and deeper ones; Add (accum 1)
+# is the LLT's, Replace (accum 0) skips the old-tile load
+for (n, k, accum) in [(16128, 128, 1), (16128, 256, 1), (16128, 512, 1), (16128, 768, 1), (16128, 1024, 1),
+                      (16128, 128, 0), (16128, 256, 0), (16128, 512, 0), (16128, 1024, 0),
+                      (12288, 256, 1), (10240, 512, 1), (8192, 256, 1), (4096, 256, 1), (1024, 256, 1), (6016, 128, 1),
+                      (3072, 128, 1)]:
     P = torch.randn((k, n), dtype=torch.float64, device=dev).T
     Cm = torch.randn((n, n), dtype=torch.float64, device=dev).T
-    line = f"{tag} SYRK(lower) n={n} k={k}:"
+    line = f"{tag} SYRK(lower, {'Add' if accum else 'Replace'}) n={n} k={k}:"
     for mode in (0, 2, 3):
         lib.faer_b200_set_option(b"gemm_ws", mode)
-        ms = best(lambda: la.matmul_triangular(Cm, 1, 1, P, 0, P.T, 0, -1.0))
+        ms = best(lambda: la.matmul_triangular(Cm, 1, accum, P, 0, P.T, 0, -1.0))
         line += f"  mode {mode}: {ms:.3f} ms {n * n * k / ms / 1e9:.2f} TF"
     print(line, flush=True)
     del P, Cm
