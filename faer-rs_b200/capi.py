@@ -192,6 +192,28 @@ class FullPivLuStatus(C.Structure):
     _fields_ = [("tag", C.c_int), ("body", _FullPivLuBody)]
 
 
+class LbltParams(C.Structure):
+    """faer.h:156-160; `pivoting` is a PIVOTING_* value."""
+    _fields_ = [("pivoting", C.c_int), ("par_threshold", C.c_size_t), ("block_size", C.c_size_t)]
+
+
+class _LbltOkBody(C.Structure):
+    _fields_ = [("transposition_count", C.c_size_t)]
+
+
+class _LbltBody(C.Union):
+    _fields_ = [("ok", _LbltOkBody)]
+
+
+class LbltStatus(C.Structure):
+    """tag: 0 Ok{transposition_count}, 1 Unknown (faer.h:324-338); 16 bytes, body at 8."""
+    _anonymous_ = ("body",)
+    _fields_ = [("tag", C.c_int), ("body", _LbltBody)]
+
+
+# faer-ffi `PivotingStrategy` discriminants (faer-ffi/src/lib.rs:492-508)
+PIVOTING_PARTIAL, PIVOTING_PARTIAL_DIAG, PIVOTING_ROOK, PIVOTING_ROOK_DIAG, PIVOTING_FULL = range(5)
+
 ACCUM_REPLACE, ACCUM_ADD = 0, 1
 CONJ_NO, CONJ_YES = 0, 1
 PAR_SEQ, PAR_RAYON = 0, 1
@@ -455,6 +477,30 @@ def load() -> C.CDLL:
                 f.restype = Layout
                 f = getattr(lib, f"libfaer_v0_23_piv_llt_{name}_{it}_{suf}")
                 f.argtypes = [MatMut, MatRef, SliceMut, SliceMut, P, MemAlloc]
+                f.restype = None
+    for suf in ("f64", "f32", "c64", "c32"):
+        getattr(lib, f"libfaer_v0_23_LbltParams_{suf}").argtypes = []
+        getattr(lib, f"libfaer_v0_23_LbltParams_{suf}").restype = LbltParams
+        for it in ("u32", "u64"):
+            pre = "libfaer_v0_23_lblt_"
+            f = getattr(lib, f"{pre}factor_in_place_scratch_{it}_{suf}")
+            f.argtypes = [C.c_size_t, P, LbltParams]
+            f.restype = Layout
+            f = getattr(lib, f"{pre}factor_in_place_{it}_{suf}")
+            f.argtypes = [MatMut, VecMut, SliceMut, SliceMut, P, MemAlloc, LbltParams]
+            f.restype = LbltStatus
+            f = getattr(lib, f"{pre}solve_in_place_scratch_{it}_{suf}")
+            f.argtypes = [C.c_size_t, C.c_size_t, P]
+            f.restype = Layout
+            f = getattr(lib, f"{pre}solve_in_place_{it}_{suf}")
+            f.argtypes = [MatRef, VecMut, VecMut, C.c_int, SliceMut, SliceMut, MatMut, P, MemAlloc]
+            f.restype = None
+            for name in ("reconstruct", "inverse"):
+                f = getattr(lib, f"{pre}{name}_scratch_{it}_{suf}")
+                f.argtypes = [C.c_size_t, P]
+                f.restype = Layout
+                f = getattr(lib, f"{pre}{name}_{it}_{suf}")
+                f.argtypes = [MatMut, MatRef, VecMut, VecMut, SliceMut, SliceMut, P, MemAlloc]
                 f.restype = None
     for suf in ("f64", "f32", "c64", "c32"):
         getattr(lib, f"libfaer_v0_23_ColPivQrParams_{suf}").argtypes = []

@@ -33,6 +33,7 @@
 
 #include "ffi_common.cuh"
 #include "panel_common.cuh"
+#include "pivot_record.cuh"
 #include "runtime.cuh"
 #include "tensor_ops.cuh"
 
@@ -135,13 +136,7 @@ __device__ __forceinline__ Fs<R> frecip(Fs<R> x) {
   return Fs<R>{fpl_mul(fpl_mul(a, inv), big), fpl_mul(fpl_mul(-b, inv), big)};
 }
 
-// per-CTA argmax record: the score and the column-major index i + j * m in X
-template <class R>
-struct alignas(16) FplRec {
-  R score;
-  long long idx;
-};
-
+// per-CTA argmax record (pivot_record.cuh): the score and the column-major index i + j * m in X
 template <class R>
 struct FplWs {
   FplRec<R>* rec;           // [grid]
@@ -150,26 +145,6 @@ struct FplWs {
   int* hist;                // [2 size]: row transposition, then column transposition of X at step k
   unsigned long long* bar;  // grid barrier counter (zeroed before the launch)
 };
-
-// (v2, i2) beats (v1, i1): larger score, then, between equal POSITIVE scores, the smaller index. "None" is (0, LLONG_MAX) and a
-// candidate must be > 0 to replace it, so the result is the first maximum in X's column-major order with strict `>` from 0 —
-// best_in_matrix_fallback's — whatever the combination order.
-template <class R>
-__device__ __forceinline__ bool fpl_better(R v2, long long i2, R v1, long long i1) {
-  return v2 > v1 || (v2 == v1 && v1 > R(0) && i2 < i1);
-}
-template <class R>
-__device__ __forceinline__ void fpl_warp_argmax(R& v, long long& i) {
-#pragma unroll
-  for (int off = 16; off > 0; off >>= 1) {
-    const R v2 = __shfl_xor_sync(0xffffffffu, v, off);
-    const long long i2 = __shfl_xor_sync(0xffffffffu, i, off);
-    if (fpl_better(v2, i2, v, i)) {
-      v = v2;
-      i = i2;
-    }
-  }
-}
 
 // The whole factorization of the column-major m x n working matrix X (leading dimension ld); tr: row k of X is the scaled side.
 template <class R, bool CX>

@@ -29,6 +29,7 @@
 
 #include "ffi_common.cuh"
 #include "panel_common.cuh"
+#include "piv_common.cuh"
 #include "runtime.cuh"
 #include "tensor_ops.cuh"
 
@@ -417,6 +418,40 @@ inline unsigned piv_blocks(i64 elems) { return (unsigned)((elems + 255) / 256); 
 
 }  // namespace
 
+// ---- piv_common.cuh: the one entry to the kernels above, for this file and lblt.cu ----
+template <class R, bool CX>
+void piv_laswp_t(cudaStream_t st, View<R> A, i64 k, i64 nt, const long long* hist) {
+  if (k == 0 || nt == 0) return;
+  piv_llt_laswp_kernel<R, CX><<<piv_blocks(k), 256, 0, st>>>(A.ptr, A.rs, A.cs, (int)k, (int)nt, hist);
+  FB_CUDA_CHECK(cudaGetLastError());
+  note_launch();
+}
+template <class R, bool CX>
+void piv_gather_rows_t(cudaStream_t st, View<R> dst, View<const R> src, const long long* perm) {
+  const i64 n = dst.nrows, k = dst.ncols;
+  if (n == 0 || k == 0) return;
+  piv_gather_rows_kernel<R, CX><<<piv_blocks(n * k), 256, 0, st>>>(dst.ptr, dst.rs, dst.cs, src.ptr, src.rs, src.cs, n, k, perm);
+  FB_CUDA_CHECK(cudaGetLastError());
+  note_launch();
+}
+template <class R, bool CX>
+void piv_sym_gather_t(cudaStream_t st, View<R> out, const R* tmp, i64 ld, const long long* p) {
+  const i64 n = out.nrows;
+  if (n == 0) return;
+  piv_sym_gather_kernel<R, CX><<<piv_blocks(n * n), 256, 0, st>>>(out.ptr, out.rs, out.cs, tmp, ld, n, p);
+  FB_CUDA_CHECK(cudaGetLastError());
+  note_launch();
+}
+#define FB_PIV_COMMON_INST(R, CX)                                                                          \
+  template void piv_laswp_t<R, CX>(cudaStream_t, View<R>, i64, i64, const long long*);                      \
+  template void piv_gather_rows_t<R, CX>(cudaStream_t, View<R>, View<const R>, const long long*);           \
+  template void piv_sym_gather_t<R, CX>(cudaStream_t, View<R>, const R*, i64, const long long*);
+FB_PIV_COMMON_INST(double, false)
+FB_PIV_COMMON_INST(float, false)
+FB_PIV_COMMON_INST(double, true)
+FB_PIV_COMMON_INST(float, true)
+#undef FB_PIV_COMMON_INST
+
 struct PivLltResult {
   int state;  // 0 Ok, 1 NonPositivePivot
   i64 index;  // the failing column, or the rank
@@ -478,11 +513,7 @@ PivLltResult piv_llt_in_place_t(cudaStream_t st, View<R> A, i64 block_size, std:
       FB_CUDA_CHECK(cudaLaunchCooperativeKernel((void*)piv_llt_panel_kernel<R, CX>, dim3(G), dim3(PIV_THREADS), args, 0, st));
       note_launch();
     }
-    if (k > 0) {
-      piv_llt_laswp_kernel<R, CX><<<piv_blocks(k), 256, 0, st>>>(A.ptr, A.rs, A.cs, (int)k, b, w.hist);
-      FB_CUDA_CHECK(cudaGetLastError());
-      note_launch();
-    }
+    piv_laswp_t<R, CX>(st, A, k, b, w.hist);
     if (k + b < n) {
       const i64 m = n - k - b;
       View<R> P = piv_sub<R, CX>(A, k + b, k, m, b);
@@ -520,13 +551,9 @@ void piv_llt_solve_t(cudaStream_t st, View<const R> L, const long long* perm, co
   FB_CUDA_CHECK(cudaMemcpyAsync(d_p, perm, (size_t)n * 8, cudaMemcpyHostToDevice, st));
   FB_CUDA_CHECK(cudaMemcpyAsync(d_p + n, perm_inv, (size_t)n * 8, cudaMemcpyHostToDevice, st));
   View<R> X{tmp, n, k, 1, n};
-  piv_gather_rows_kernel<R, CX><<<piv_blocks(n * k), 256, 0, st>>>(tmp, 1, n, rhs.ptr, rhs.rs, rhs.cs, n, k, d_p);
-  FB_CUDA_CHECK(cudaGetLastError());
-  note_launch();
+  piv_gather_rows_t<R, CX>(st, X, View<const R>{rhs.ptr, n, k, rhs.rs, rhs.cs}, d_p);
   piv_llt_solve(st, L, conj, X, Tag());
-  piv_gather_rows_kernel<R, CX><<<piv_blocks(n * k), 256, 0, st>>>(rhs.ptr, rhs.rs, rhs.cs, tmp, 1, n, n, k, d_p + n);
-  FB_CUDA_CHECK(cudaGetLastError());
-  note_launch();
+  piv_gather_rows_t<R, CX>(st, rhs, View<const R>{tmp, n, k, 1, n}, d_p + n);
   FB_CUDA_CHECK(cudaStreamSynchronize(st));  // the host permutations and the pool buffers are released below
   ws_free(tmp);
   ws_free(d_p);
@@ -544,9 +571,7 @@ void piv_llt_recon_t(cudaStream_t st, View<R> out, View<const R> L, const long l
   R* tmp = (R*)ws_alloc((size_t)n * (size_t)n * W * sizeof(R));
   FB_CUDA_CHECK(cudaMemcpyAsync(d_p, perm_inv, (size_t)n * 8, cudaMemcpyHostToDevice, st));
   piv_llt_product<R, CX>(st, View<R>{tmp, n, n, 1, n}, L, inverse);
-  piv_sym_gather_kernel<R, CX><<<piv_blocks(n * n), 256, 0, st>>>(out.ptr, out.rs, out.cs, tmp, n, n, d_p);
-  FB_CUDA_CHECK(cudaGetLastError());
-  note_launch();
+  piv_sym_gather_t<R, CX>(st, out, tmp, n, d_p);
   FB_CUDA_CHECK(cudaStreamSynchronize(st));
   ws_free(tmp);
   ws_free(d_p);

@@ -18,7 +18,8 @@ import numpy as np
 
 from . import capi
 from .capi import (ACCUM_ADD, ACCUM_REPLACE, BLOCK_LOWER, BLOCK_RECT, BLOCK_STRICT_LOWER, BLOCK_STRICT_UPPER,  # noqa: F401
-                   BLOCK_UNIT_LOWER, BLOCK_UNIT_UPPER, BLOCK_UPPER, CONJ_NO, CONJ_YES)
+                   BLOCK_UNIT_LOWER, BLOCK_UNIT_UPPER, BLOCK_UPPER, CONJ_NO, CONJ_YES, PIVOTING_FULL, PIVOTING_PARTIAL,
+                   PIVOTING_PARTIAL_DIAG, PIVOTING_ROOK, PIVOTING_ROOK_DIAG)
 
 
 class Accum:
@@ -771,6 +772,80 @@ def piv_llt_inverse(out, L, perm, perm_inv, par=None) -> None:
     getattr(capi.load(), f"libfaer_v0_23_piv_llt_inverse_{_perm_width(perm)}_{suf}")(
         capi.mat_mut(out), capi.mat_ref(L), capi.slice_mut(perm), capi.slice_mut(perm_inv), par or capi.par_default(),
         capi.MemAlloc(None, 0))
+
+
+# ---- Bunch-Kaufman LBLT (cholesky::lblt) -----------------------------------------------------------
+@dataclass
+class LbltInfo:
+    transposition_count: int
+
+
+def lblt_params_default():
+    """LbltParams { pivoting: PartialDiag, par_threshold: 128 * 128, block_size: 64 } (bunch_kaufman/factor.rs:903-910)."""
+    return capi.load().libfaer_v0_23_LbltParams_f64()
+
+
+def _vec(x, n, like):
+    """A VecRef / VecMut over a 1-D numpy array or torch tensor of `like`'s dtype, or (x a 2-D matrix) over its diagonal."""
+    if capi._is_torch(x):
+        if x.dim() == 2:
+            return capi.VecMut(x.data_ptr(), n, x.stride(0) + x.stride(1))
+        assert x.dim() == 1 and x.numel() == n and x.dtype == like.dtype
+        return capi.VecMut(x.data_ptr(), n, x.stride(0))
+    if x.ndim == 2:
+        return capi.VecMut(x.ctypes.data, n, (x.strides[0] + x.strides[1]) // x.itemsize)
+    assert x.ndim == 1 and x.size == n and x.dtype == like.dtype
+    return capi.VecMut(x.ctypes.data, n, x.strides[0] // x.itemsize)
+
+
+def lblt_in_place(A, subdiag, perm, perm_inv, params=None, par=None) -> LbltInfo:
+    """cholesky::lblt::factor::cholesky_in_place (bunch_kaufman/factor.rs:1161-1234): P A P^T = L B L^H of the self-adjoint A
+    (lower triangle), in place: L strictly below the diagonal, B's diagonal on it, B's subdiagonal in `subdiag` (a 1-D array or
+    tensor of A's dtype; pass it zeroed: entries of 1 x 1 blocks with a zero column are left as given). `perm`/`perm_inv`:
+    uint32/uint64 arrays (numpy) or int32/int64 CUDA tensors; (P A P^T)[i, j] = A[perm[i], perm[j]]. PIVOTING_FULL also
+    scales the strict upper triangle (see include/faer_b200_lblt.h)."""
+    lib = capi.load()
+    suf = _suf_lu(A)
+    params = params or getattr(lib, f"libfaer_v0_23_LbltParams_{suf}")()
+    par = par or capi.par_default()
+    it = _perm_width(perm)
+    n = A.shape[0]
+    lay = getattr(lib, f"libfaer_v0_23_lblt_factor_in_place_scratch_{it}_{suf}")(n, par, params)
+    scratch = np.empty(lay.len_bytes + lay.align_bytes, dtype=np.uint8)
+    st = getattr(lib, f"libfaer_v0_23_lblt_factor_in_place_{it}_{suf}")(
+        capi.mat_mut(A), _vec(subdiag, n, A), capi.slice_mut(perm), capi.slice_mut(perm_inv), par,
+        capi.MemAlloc(scratch.ctypes.data, scratch.size), params)
+    if st.tag != 0:
+        raise RuntimeError("LbltStatus::Unknown")
+    return LbltInfo(int(st.ok.transposition_count))
+
+
+def lblt_solve_in_place(L, subdiag, perm, perm_inv, rhs, conj: int = CONJ_NO, par=None, diag=None) -> None:
+    """cholesky::lblt::solve::solve_in_place_with_conj (bunch_kaufman/solve.rs:35-104): rhs <- A^-1 rhs (conj(A)^-1 rhs with
+    CONJ_YES). `diag` defaults to L's diagonal."""
+    suf = _same_suffix(L, rhs)
+    n = L.shape[0]
+    getattr(capi.load(), f"libfaer_v0_23_lblt_solve_in_place_{_perm_width(perm)}_{suf}")(
+        capi.mat_ref(L), _vec(L if diag is None else diag, n, L), _vec(subdiag, n, L), conj, capi.slice_mut(perm),
+        capi.slice_mut(perm_inv), capi.mat_mut(rhs), par or capi.par_default(), capi.MemAlloc(None, 0))
+
+
+def lblt_reconstruct(out, L, subdiag, perm, perm_inv, par=None, diag=None) -> None:
+    """cholesky::lblt::reconstruct (bunch_kaufman/reconstruct.rs:12-87): every entry of out is written; its LOWER triangle is A."""
+    suf = _same_suffix(out, L)
+    n = L.shape[0]
+    getattr(capi.load(), f"libfaer_v0_23_lblt_reconstruct_{_perm_width(perm)}_{suf}")(
+        capi.mat_mut(out), capi.mat_ref(L), _vec(L if diag is None else diag, n, L), _vec(subdiag, n, L), capi.slice_mut(perm),
+        capi.slice_mut(perm_inv), par or capi.par_default(), capi.MemAlloc(None, 0))
+
+
+def lblt_inverse(out, L, subdiag, perm, perm_inv, par=None, diag=None) -> None:
+    """cholesky::lblt::inverse (bunch_kaufman/inverse.rs:11-42): out <- A^-1 (all n^2 entries)."""
+    suf = _same_suffix(out, L)
+    n = L.shape[0]
+    getattr(capi.load(), f"libfaer_v0_23_lblt_inverse_{_perm_width(perm)}_{suf}")(
+        capi.mat_mut(out), capi.mat_ref(L), _vec(L if diag is None else diag, n, L), _vec(subdiag, n, L), capi.slice_mut(perm),
+        capi.slice_mut(perm_inv), par or capi.par_default(), capi.MemAlloc(None, 0))
 
 
 # ---- column-pivoted QR (qr::col_pivoting) ----------------------------------------------------------

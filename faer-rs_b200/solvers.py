@@ -332,6 +332,70 @@ class Ldlt(_Solve):
         return mul(LDm, _adjoint(self._L))
 
 
+class Lblt(_Solve):
+    """P A P^T = L B L^H, Bunch-Kaufman pivoting (solvers.rs Lblt): the factored matrix holds L strictly below the diagonal and
+    B's diagonal on it, `subdiag()` B's subdiagonal (zeroed before the factorization, as the reference does). Factors the
+    indefinite self-adjoint matrices that Ldlt cannot, such as saddle-point systems. `P()` returns (perm_fwd, perm_bwd)."""
+
+    def __init__(self, LB, sub, fwd, bwd):
+        self._LB, self._sub, self._fwd, self._bwd = LB, sub, fwd, bwd
+
+    @classmethod
+    def new(cls, A, side: int = Side.Lower, params=None) -> "Lblt":
+        assert A.ndim == 2 and A.shape[0] == A.shape[1]
+        n = A.shape[0]
+        LB = _zeros(A, n, n)
+        _assign(LB, _tri(A if side == Side.Lower else _adjoint(A), lower=True))
+        if _t(LB):
+            import torch
+            sub = torch.zeros(n, dtype=LB.dtype, device=LB.device)
+            fwd, bwd = (torch.zeros(n, dtype=torch.int64, device=LB.device) for _ in range(2))
+        else:
+            sub = np.zeros(n, dtype=LB.dtype)
+            fwd, bwd = np.zeros(n, dtype=np.uint64), np.zeros(n, dtype=np.uint64)
+        la.lblt_in_place(LB, sub, fwd, bwd, params=params)
+        return cls(LB, sub, fwd, bwd)
+
+    def LB(self):
+        return self._LB
+
+    def subdiag(self):
+        return self._sub
+
+    def P(self):
+        return self._fwd, self._bwd
+
+    def nrows(self) -> int:
+        return self._LB.shape[0]
+
+    ncols = nrows
+
+    def _like(self):
+        return self._LB
+
+    def _solve_core(self, rhs, conj: int) -> None:
+        la.lblt_solve_in_place(self._LB, self._sub, self._fwd, self._bwd, rhs, conj)
+
+    def _solve_transpose_core(self, rhs, conj: int) -> None:
+        # A^T = conj(A) for a self-adjoint A: conj composed with Yes (as Llt above)
+        la.lblt_solve_in_place(self._LB, self._sub, self._fwd, self._bwd, rhs, la.CONJ_NO if conj == la.CONJ_YES else la.CONJ_YES)
+
+    def reconstruct(self):
+        """bunch_kaufman/reconstruct.rs: the lower triangle of A, mirrored (make_self_adjoint)."""
+        n = self.nrows()
+        out = _zeros(self._LB, n, n)
+        la.lblt_reconstruct(out, self._LB, self._sub, self._fwd, self._bwd)
+        _assign(out, _tri(out, lower=True) + _adjoint(_tri(out, lower=True, k=-1)))
+        return out
+
+    def inverse(self):
+        """bunch_kaufman/inverse.rs."""
+        n = self.nrows()
+        out = _zeros(self._LB, n, n)
+        la.lblt_inverse(out, self._LB, self._sub, self._fwd, self._bwd)
+        return out
+
+
 class PartialPivLu(_Solve):
     """P A = L U (solvers.rs:981-1034). `P()` returns (perm_fwd, perm_bwd): (P A)[i, :] = A[perm_fwd[i], :]."""
 
@@ -713,6 +777,10 @@ def llt(A, side: int = Side.Lower) -> Llt:
 
 def ldlt(A, side: int = Side.Lower) -> Ldlt:
     return Ldlt.new(A, side)
+
+
+def lblt(A, side: int = Side.Lower) -> Lblt:
+    return Lblt.new(A, side)
 
 
 def partial_piv_lu(A) -> PartialPivLu:

@@ -717,5 +717,7 @@ void libfaer_v0_23_partial_piv_lu_solve_transpose_in_place_u64_c32(struct FaerV0
 #include "faer_b200_colpiv_qr.h"
 /* full-pivoting LU (full_piv_lu_*): declared in its own header */
 #include "faer_b200_full_piv_lu.h"
+/* Bunch-Kaufman LBLT (lblt_*): declared in its own header */
+#include "faer_b200_lblt.h"
 
 #endif /* LIBFAER_V0_24 */
