@@ -92,6 +92,30 @@ class EvdStatus(C.Structure):
     _fields_ = [("tag", C.c_int), ("body", _StatusBody)]
 
 
+class HessenbergParams(C.Structure):
+    """faer.h:110-113."""
+    _fields_ = [("par_threshold", C.c_size_t), ("blocking_threshold", C.c_size_t)]
+
+
+SHIFT_COUNT_FN = C.CFUNCTYPE(C.c_size_t, C.c_size_t, C.c_size_t)
+
+
+class SchurParams(C.Structure):
+    """faer.h:115-120; the two callbacks run on the host."""
+    _fields_ = [("recommended_shift_count", SHIFT_COUNT_FN), ("recommended_deflation_window", SHIFT_COUNT_FN),
+                ("blocking_threshold", C.c_size_t), ("nibble_threshold", C.c_size_t)]
+
+
+class EvdFromSchurParams(C.Structure):
+    """faer.h:106-108."""
+    _fields_ = [("recursion_threshold", C.c_size_t)]
+
+
+class EvdParams(C.Structure):
+    """faer.h:122-126."""
+    _fields_ = [("hessenberg", HessenbergParams), ("schur", SchurParams), ("evd_from_schur", EvdFromSchurParams)]
+
+
 class BidiagParams(C.Structure):
     _fields_ = [("par_threshold", C.c_size_t)]
 
@@ -328,6 +352,18 @@ def load() -> C.CDLL:
         f = getattr(lib, f"libfaer_v0_23_self_adjoint_evd_{suf}")
         f.argtypes = [MatRef, MatMut, VecMut, P, MemAlloc, SelfAdjointEvdParams]
         f.restype = EvdStatus
+    for suf in ("f64", "f32", "c64", "c32"):
+        for name, ty in (("EvdFromSchurParams", EvdFromSchurParams), ("SchurParams", SchurParams), ("EvdParams", EvdParams)):
+            getattr(lib, f"libfaer_v0_23_{name}_{suf}").argtypes = []
+            getattr(lib, f"libfaer_v0_23_{name}_{suf}").restype = ty
+        f = getattr(lib, f"libfaer_v0_23_evd_scratch_{suf}")
+        f.argtypes = [C.c_size_t, C.c_int, C.c_int, P, EvdParams]
+        f.restype = Layout
+        f = getattr(lib, f"libfaer_v0_23_evd_{suf}")
+        f.argtypes = [MatRef, MatMut, MatMut, VecMut, VecMut, P, MemAlloc, EvdParams]
+        f.restype = EvdStatus
+    lib.faer_b200_evd_last_sweep_counts.argtypes = [C.POINTER(C.c_longlong)]
+    lib.faer_b200_evd_last_sweep_counts.restype = None
     for suf in ("f64", "f32", "c64", "c32"):
         for name in ("inverse_triangular_lower", "inverse_triangular_upper", "inverse_unit_triangular_lower", "inverse_unit_triangular_upper"):
             f = getattr(lib, f"libfaer_v0_23_{name}_in_place_{suf}")

@@ -92,6 +92,13 @@ void tridiag_in_place_cx(cudaStream_t st, View<TO> A, View<TO> H);
 // <float, false> f32, <double, true> c64, <float, true> c32 (complex views in complex units)
 template <class TO, bool CX>
 void hessenberg_in_place_t(cudaStream_t st, View<TO> A, View<TO> Hf);
+// ---- schur.cu: general eigendecomposition (evd/mod.rs:1007-1246). <TO, complex?> as above; UL / UR with ptr == nullptr: not
+// computed; S / S_im: device, compact, n entries of TO's kind (S_im: real kinds only). ns_limit bounds the shifts of a sweep. False
+// on a non-finite input (nothing written) or when the iteration cap is reached. ----
+template <class TO, bool CX>
+bool evd_general(cudaStream_t st, View<const TO> A, View<TO> UL, View<TO> UR, TO* S, TO* S_im, size_t ns_limit);
+// sweeps and chased windows of the last evd_general call (tools/time_evd.py)
+extern long long g_evd_last_sweeps, g_evd_last_windows;
 // ---- tridiag_dc.cu: divide-and-conquer eigensolver of a symmetric tridiagonal matrix (device arrays) ----
 bool tridiag_dc_f64(cudaStream_t st, const double* d, const double* e, i64 n, double* lam, double* Q, i64 ldq);
 // ---- tridiag.cu ----

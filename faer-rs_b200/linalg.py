@@ -659,6 +659,33 @@ def self_adjoint_evd(A, S, U=None, par=None, params=None) -> None:
         S[...] = tmp.real
 
 
+def evd(A, S, S_im=None, UL=None, UR=None, par=None, params=None) -> None:
+    """evd::evd_real / evd_cplx (evd/mod.rs:1180-1246) through `libfaer_v0_23_evd_<T>`: the eigenvalues of a general square A and,
+    when given, its left (UL) and right (UR) eigenvectors, n x n each. Real A: eigenvalue k is S[k] + i S_im[k]; a conjugate pair
+    sits at k, k + 1 with S_im[k] > 0 and its eigenvectors are column k +- i column k + 1. Complex A: S only (A's dtype).
+    f64 / f32 / c64 / c32 (f32 / c32 compute in f64 / c64). Raises RuntimeError("EvdError::NoConvergence") on non-finite input
+    or when the sweep cap is reached; the outputs are then as they were."""
+    lib = capi.load()
+    suf = _suf_lu(A)
+    n = A.shape[0]
+    cx = suf in ("c64", "c32")
+    assert A.shape[1] == n and S.shape == (n,) and S.dtype == A.dtype
+    if not cx:
+        assert S_im is not None and S_im.shape == (n,) and S_im.dtype == A.dtype
+
+    def vec(v):
+        return capi.VecMut(v.data_ptr() if capi._is_torch(v) else v.ctypes.data, n, 1)
+
+    none = capi.MatMut(None, 0, 0, 0, 0)
+    params = params or getattr(lib, f"libfaer_v0_23_EvdParams_{suf}")()
+    st = getattr(lib, f"libfaer_v0_23_evd_{suf}")(capi.mat_ref(A), capi.mat_mut(UL) if UL is not None else none,
+                                                  capi.mat_mut(UR) if UR is not None else none, vec(S),
+                                                  vec(S_im) if not cx else capi.VecMut(None, 0, 1), par or capi.par_default(),
+                                                  capi.MemAlloc(None, 0), params)
+    if st.tag != 0:
+        raise RuntimeError("EvdError::NoConvergence")
+
+
 def bidiag_in_place(A, H_left, H_right, par=None, params=None) -> None:
     """svd::bidiag::bidiag_in_place (svd/bidiag.rs:47-256): A = U B V^H for nrows >= ncols, f64 / f32 (HBM-bound kernels) or c64 / c32 (functional). B ends up on A's
     diagonal / superdiagonal, the left reflectors below the diagonal (T blocks in H_left, bl x ncols), the right

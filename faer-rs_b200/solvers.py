@@ -758,6 +758,42 @@ class SelfAdjointEigen:
         return self._S
 
 
+class Eigen:
+    """`Eigen<T>` (solvers.rs: `Eigen::new`, `new_from_real`, `new_from_complex`): A U = U diag(S) for a general square A, with U
+    and S complex also for real A (a real conjugate pair's packed columns k, k + 1 become column k +- i column k + 1)."""
+
+    def __init__(self, U, S):
+        self._U, self._S = U, S
+
+    @classmethod
+    def new(cls, A):
+        n = A.shape[0]
+        UR = la._new_mat(A, n, n)
+        if capi._is_torch(A):
+            import torch
+            S, S_im = (torch.zeros(n, dtype=A.dtype, device=A.device) for _ in range(2))
+            cx = A.dtype.is_complex
+        else:
+            S, S_im = np.zeros(n, dtype=A.dtype), np.zeros(n, dtype=A.dtype)
+            cx = np.iscomplexobj(A)
+        la.evd(A, S, None if cx else S_im, None, UR)
+        if cx:
+            return cls(UR, S)
+        U = UR + 0j * UR
+        first = S_im > 0
+        second = S_im < 0
+        im = UR[:, 1:][:, first[:-1]]
+        U[:, first] = UR[:, first] + 1j * im
+        U[:, second] = UR[:, first] - 1j * im
+        return cls(U, S + 1j * S_im)
+
+    def U(self):
+        return self._U
+
+    def S(self):
+        return self._S
+
+
 def svd(A) -> Svd:
     return Svd.new(A)
 
@@ -802,6 +838,24 @@ def colpiv_qr(A) -> ColPivQr:
 def singular_values(A):
     """`A.singular_values()` (solvers.rs:457-487): non-increasing, through `svd` with no vectors."""
     return la.singular_values(A)
+
+
+def eigen(A) -> Eigen:
+    return Eigen.new(A)
+
+
+def eigenvalues(A):
+    """`A.eigenvalues()` (solvers.rs): complex, through `evd` with no vectors."""
+    n = A.shape[0]
+    if capi._is_torch(A):
+        import torch
+        S, S_im = (torch.zeros(n, dtype=A.dtype, device=A.device) for _ in range(2))
+        cx = A.dtype.is_complex
+    else:
+        S, S_im = np.zeros(n, dtype=A.dtype), np.zeros(n, dtype=A.dtype)
+        cx = np.iscomplexobj(A)
+    la.evd(A, S, None if cx else S_im)
+    return S if cx else S + 1j * S_im
 
 
 def self_adjoint_eigenvalues(A, side: int = Side.Lower):
