@@ -34,7 +34,10 @@
 
 #include "ffi_common.cuh"
 #include "panel_common.cuh"
+#include "piv_common.cuh"
+#include "pivot_record.cuh"
 #include "runtime.cuh"
+#include "scalar.cuh"
 #include "tensor_ops.cuh"
 
 namespace fb {
@@ -46,80 +49,14 @@ constexpr int CPQ_WARPS = CPQ_THREADS / 32;
 constexpr int CPQ_MIN_SEG = 256;  // shortest row segment of a split column
 constexpr int CPQ_REC = 4;        // stride of a partial record (3 norm accumulators, or one scalar)
 
-template <class R>
-struct CpqLim;
-template <>
-struct CpqLim<double> {
-  __device__ static double sml() { return 0x1p-511; }
-  __device__ static double big() { return 0x1p511; }
-};
-template <>
-struct CpqLim<float> {
-  __device__ static float sml() { return 0x1p-63f; }
-  __device__ static float big() { return 0x1p63f; }
-};
-
-// a scalar of the kind: (re, im), im == 0 for the real types
-template <class R>
-struct Sc {
-  R re, im;
-};
-template <class R, bool CX>
-__device__ __forceinline__ Sc<R> ldx(const R* p) {
-  return Sc<R>{__ldcg(p), CX ? __ldcg(p + 1) : R(0)};
-}
-template <class R, bool CX>
-__device__ __forceinline__ void stx(R* p, Sc<R> v) {
-  p[0] = v.re;
-  if (CX) p[1] = v.im;
-}
-template <class R, bool CX>
-__device__ __forceinline__ Sc<R> cmul(Sc<R> a, Sc<R> b) {
-  if (!CX) return Sc<R>{a.re * b.re, R(0)};
-  return Sc<R>{a.re * b.re - a.im * b.im, a.re * b.im + a.im * b.re};
-}
-// acc + conj(a) * b
-template <class R, bool CX>
-__device__ __forceinline__ Sc<R> conj_mul_add(Sc<R> a, Sc<R> b, Sc<R> acc) {
-  acc.re = fma(a.re, b.re, acc.re);
-  if (CX) {
-    acc.re = fma(a.im, b.im, acc.re);
-    acc.im = fma(a.re, b.im, acc.im);
-    acc.im = fma(-a.im, b.re, acc.im);
-  }
-  return acc;
-}
-// acc + a * b
-template <class R, bool CX>
-__device__ __forceinline__ Sc<R> mul_add(Sc<R> a, Sc<R> b, Sc<R> acc) {
-  acc.re = fma(a.re, b.re, acc.re);
-  if (CX) {
-    acc.re = fma(-a.im, b.im, acc.re);
-    acc.im = fma(a.re, b.im, acc.im);
-    acc.im = fma(a.im, b.re, acc.im);
-  }
-  return acc;
-}
-template <class R, bool CX>
-__device__ __forceinline__ Sc<R> cadd(Sc<R> a, Sc<R> b) {
-  return Sc<R>{a.re + b.re, CX ? a.im + b.im : R(0)};
-}
-template <class R, bool CX>
-__device__ __forceinline__ Sc<R> scale(Sc<R> a, R s) {
-  return Sc<R>{a.re * s, CX ? a.im * s : R(0)};
-}
-template <class R, bool CX>
-__device__ __forceinline__ R abs2(Sc<R> a) {
-  return CX ? a.re * a.re + a.im * a.im : a.re * a.re;
-}
 template <class R, bool CX>
 __device__ __forceinline__ void acc_norm(NormAcc<R>& a, Sc<R> x) {
-  a.add(x.re, CpqLim<R>::sml(), CpqLim<R>::big());
-  if (CX) a.add(x.im, CpqLim<R>::sml(), CpqLim<R>::big());
+  a.add(x.re, TLim<R>::sqrt_min(), TLim<R>::sqrt_max());
+  if (CX) a.add(x.im, TLim<R>::sqrt_min(), TLim<R>::sqrt_max());
 }
 template <class R>
 __device__ __forceinline__ R acc_value(R s, R m, R b) {
-  return norm_from_acc(s, m, b, CpqLim<R>::sml(), CpqLim<R>::big());
+  return norm_from_acc(s, m, b, TLim<R>::sqrt_min(), TLim<R>::sqrt_max());
 }
 
 template <class R>
@@ -146,13 +83,9 @@ __device__ __forceinline__ Split make_split(i64 nc, i64 nr, int warps) {
   return s;
 }
 
-// (v2, i2) beats (v1, i1): larger value, then, between equal POSITIVE values, the smaller column. "None" is (0, INT_MAX) and a
-// candidate must be > 0 to replace it, so the result is the reference's first maximum with strict `>` from 0 (factor.rs:161-169,
-// 186-193) whatever the combination order: a norm of exactly 0 or NaN is never chosen, and "none" leaves the caller's default.
-template <class R>
-__device__ __forceinline__ bool cpq_better(R v2, int i2, R v1, int i1) { return v2 > v1 || (v2 == v1 && v1 > R(0) && i2 < i1); }
-
-// CTA-wide first maximum; every thread gets the result
+// CTA-wide first maximum by pivot_record.cuh's `better` on (norm, column), "none" = (0, INT_MAX): the reference's first maximum
+// with strict `>` from 0 (factor.rs:161-169, 186-193); a norm of exactly 0 or NaN is never chosen, and "none" leaves the caller's
+// default. Every thread gets the result.
 template <class R>
 __device__ __forceinline__ void cta_argmax(R& v, int& i, R* sv, int* si) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -160,7 +93,7 @@ __device__ __forceinline__ void cta_argmax(R& v, int& i, R* sv, int* si) {
   for (int off = 16; off > 0; off >>= 1) {
     const R v2 = __shfl_xor_sync(0xffffffffu, v, off);
     const int i2 = __shfl_xor_sync(0xffffffffu, i, off);
-    if (cpq_better(v2, i2, v, i)) {
+    if (better(v2, i2, v, i)) {
       v = v2;
       i = i2;
     }
@@ -174,7 +107,7 @@ __device__ __forceinline__ void cta_argmax(R& v, int& i, R* sv, int* si) {
   v = sv[0];
   i = si[0];
   for (int q = 1; q < CPQ_WARPS; ++q)
-    if (cpq_better(sv[q], si[q], v, i)) {
+    if (better(sv[q], si[q], v, i)) {
       v = sv[q];
       i = si[q];
     }
@@ -222,7 +155,7 @@ __global__ void __launch_bounds__(CPQ_THREADS) colpiv_qr_kernel(R* __restrict__ 
     for (i64 u = gw; u < (i64)n * sp.S; u += warps) {
       const i64 j = u / sp.S, lo = (u % sp.S) * sp.seg, hi = min((i64)m, lo + sp.seg);
       NormAcc<R> a{R(0), R(0), R(0)};
-      for (i64 i = lo + lane; i < hi; i += 32) acc_norm<R, CX>(a, ldx<R, CX>(at(i, j)));
+      for (i64 i = lo + lane; i < hi; i += 32) acc_norm<R, CX>(a, sc_ld<R, CX>(at(i, j)));
       a.s = warp_sum(a.s);
       a.m = warp_sum(a.m);
       a.b = warp_sum(a.b);
@@ -242,7 +175,7 @@ __global__ void __launch_bounds__(CPQ_THREADS) colpiv_qr_kernel(R* __restrict__ 
     int ix = INT_MAX;
     for (int j = tid; j < n; j += CPQ_THREADS) {
       const R val = combine_norm(w.part, (i64)j * sp.S, sp.S);
-      if (cpq_better(val, j, v, ix)) {
+      if (better(val, j, v, ix)) {
         v = val;
         ix = j;
       }
@@ -273,7 +206,7 @@ __global__ void __launch_bounds__(CPQ_THREADS) colpiv_qr_kernel(R* __restrict__ 
     int best_col = INT_MAX;
     for (int j = k + tid; j < n; j += CPQ_THREADS) {
       const R val = __ldcg(w.norm + j);
-      if (cpq_better(val, j, new_best, best_col)) {
+      if (better(val, j, new_best, best_col)) {
         new_best = val;
         best_col = j;
       }
@@ -288,12 +221,12 @@ __global__ void __launch_bounds__(CPQ_THREADS) colpiv_qr_kernel(R* __restrict__ 
       const Split sp = make_split(nc, nr, warps);
       for (i64 u = gw; u < nc * sp.S; u += warps) {
         const i64 j = k + u / sp.S, lo = k + (u % sp.S) * sp.seg, hi = min((i64)m, lo + sp.seg);
-        const Sc<R> d = ldx<R, CX>(w.dot + W * j);
+        const Sc<R> d = sc_ld<R, CX>(w.dot + W * j);
         NormAcc<R> a{R(0), R(0), R(0)};
         for (i64 i = lo + lane; i < hi; i += 32) {
           R* p = at(i, j);
-          const Sc<R> x = mul_add<R, CX>(ldx<R, CX>(at(i, k - 1)), d, ldx<R, CX>(p));
-          stx<R, CX>(p, x);
+          const Sc<R> x = mul_add<R, CX>(sc_ld<R, CX>(at(i, k - 1)), d, sc_ld<R, CX>(p));
+          sc_st<R, CX>(p, x);
           acc_norm<R, CX>(a, x);
         }
         a.s = warp_sum(a.s);
@@ -312,7 +245,7 @@ __global__ void __launch_bounds__(CPQ_THREADS) colpiv_qr_kernel(R* __restrict__ 
       for (int j = k + tid; j < n; j += CPQ_THREADS) {
         const R val = combine_norm(w.part, (i64)(j - k) * sp.S, sp.S);
         if (blockIdx.x == 0) w.norm[j] = val;
-        if (cpq_better(val, j, v, ix)) {
+        if (better(val, j, v, ix)) {
           v = val;
           ix = j;
         }
@@ -324,19 +257,19 @@ __global__ void __launch_bounds__(CPQ_THREADS) colpiv_qr_kernel(R* __restrict__ 
     }
 
     // ---- P1: swap columns k / best_col, pending update of the pivot column, partial tail norms ----
-    const Sc<R> r = ldx<R, CX>(w.dot + W * best_col);  // dot[k] after the swap
+    const Sc<R> r = sc_ld<R, CX>(w.dot + W * best_col);  // dot[k] after the swap
     NormAcc<R> a{R(0), R(0), R(0)};
     for (i64 i = gt; i < m; i += T) {
       R* pk = at(i, k);
-      Sc<R> x = ldx<R, CX>(pk);
+      Sc<R> x = sc_ld<R, CX>(pk);
       if (best_col != k) {
         R* pb = at(i, best_col);
-        const Sc<R> y = ldx<R, CX>(pb);
-        stx<R, CX>(pb, x);
+        const Sc<R> y = sc_ld<R, CX>(pb);
+        sc_st<R, CX>(pb, x);
         x = y;
       }
-      if (i >= k && delayed) x = mul_add<R, CX>(r, ldx<R, CX>(at(i, k - 1)), x);
-      stx<R, CX>(pk, x);
+      if (i >= k && delayed) x = mul_add<R, CX>(r, sc_ld<R, CX>(at(i, k - 1)), x);
+      sc_st<R, CX>(pk, x);
       if (i > k) acc_norm<R, CX>(a, x);
     }
     {
@@ -353,7 +286,7 @@ __global__ void __launch_bounds__(CPQ_THREADS) colpiv_qr_kernel(R* __restrict__ 
     }
     __syncthreads();
     const R tail_norm = s_tail[0];
-    Sc<R> head = ldx<R, CX>(at(k, k));
+    Sc<R> head = sc_ld<R, CX>(at(k, k));
     R head_norm = CX ? hypot(head.re, head.im) : fabs(head.re);
     if (head_norm < TLim<R>::min_pos()) {
       head = Sc<R>{R(0), R(0)};
@@ -381,7 +314,7 @@ __global__ void __launch_bounds__(CPQ_THREADS) colpiv_qr_kernel(R* __restrict__ 
     }
     if (!no_tail)
       for (i64 i = gt; i < m; i += T)
-        if (i > k) stx<R, CX>(at(i, k), cmul<R, CX>(ldx<R, CX>(at(i, k)), inv));
+        if (i > k) sc_st<R, CX>(at(i, k), cmul<R, CX>(sc_ld<R, CX>(at(i, k)), inv));
     if (leader) {
       w.tau[k] = tau;
       w.hist[k] = best_col;
@@ -397,16 +330,16 @@ __global__ void __launch_bounds__(CPQ_THREADS) colpiv_qr_kernel(R* __restrict__ 
       }
     }
     const R tau_inv = R(1) / tau;
-    const Sc<R> l = delayed ? ldx<R, CX>(at(k, k - 1)) : Sc<R>{R(0), R(0)};  // row k of column k-1: not written in P1 / P2
+    const Sc<R> l = delayed ? sc_ld<R, CX>(at(k, k - 1)) : Sc<R>{R(0), R(0)};  // row k of column k-1: not written in P1 / P2
     barrier();
-    if (leader) stx<R, CX>(at(k, k), new_head);  // beta; every CTA has read the old head before the barrier
+    if (leader) sc_st<R, CX>(at(k, k), new_head);  // beta; every CTA has read the old head before the barrier
 
     if (k + 1 == size) {
       // factor.rs:231-240: the last reflector; the pending update reaches row k of the remaining columns only
       if (delayed)
         for (i64 j = k + 1 + gt; j < n; j += T) {
           R* p = at(k, j);
-          stx<R, CX>(p, mul_add<R, CX>(l, ldx<R, CX>(w.dot + W * j), ldx<R, CX>(p)));
+          sc_st<R, CX>(p, mul_add<R, CX>(l, sc_ld<R, CX>(w.dot + W * j), sc_ld<R, CX>(p)));
         }
       break;
     }
@@ -419,27 +352,27 @@ __global__ void __launch_bounds__(CPQ_THREADS) colpiv_qr_kernel(R* __restrict__ 
       Sc<R> acc{R(0), R(0)};
       if (delayed) {
         // update_mat_and_dot_simd: dst += v_{k-1} dot[j]; acc += v_k^H dst; dst written back
-        const Sc<R> b0 = ldx<R, CX>(w.dot + W * j);
+        const Sc<R> b0 = sc_ld<R, CX>(w.dot + W * j);
         i64 i = lo + lane;
         for (; i + 96 < hi; i += 128) {
           Sc<R> y[4], v[4], d[4];
 #pragma unroll
           for (int q = 0; q < 4; ++q) {
-            y[q] = ldx<R, CX>(at(i + 32 * q, k - 1));
-            v[q] = ldx<R, CX>(at(i + 32 * q, k));
-            d[q] = ldx<R, CX>(at(i + 32 * q, j));
+            y[q] = sc_ld<R, CX>(at(i + 32 * q, k - 1));
+            v[q] = sc_ld<R, CX>(at(i + 32 * q, k));
+            d[q] = sc_ld<R, CX>(at(i + 32 * q, j));
           }
 #pragma unroll
           for (int q = 0; q < 4; ++q) {
             d[q] = mul_add<R, CX>(y[q], b0, d[q]);
             acc = conj_mul_add<R, CX>(v[q], d[q], acc);
-            stx<R, CX>(at(i + 32 * q, j), d[q]);
+            sc_st<R, CX>(at(i + 32 * q, j), d[q]);
           }
         }
         for (; i < hi; i += 32) {
-          const Sc<R> d = mul_add<R, CX>(ldx<R, CX>(at(i, k - 1)), b0, ldx<R, CX>(at(i, j)));
-          acc = conj_mul_add<R, CX>(ldx<R, CX>(at(i, k)), d, acc);
-          stx<R, CX>(at(i, j), d);
+          const Sc<R> d = mul_add<R, CX>(sc_ld<R, CX>(at(i, k - 1)), b0, sc_ld<R, CX>(at(i, j)));
+          acc = conj_mul_add<R, CX>(sc_ld<R, CX>(at(i, k)), d, acc);
+          sc_st<R, CX>(at(i, j), d);
         }
       } else {
         // the GEMV form: acc = v_k^H B11[:, j]
@@ -448,13 +381,13 @@ __global__ void __launch_bounds__(CPQ_THREADS) colpiv_qr_kernel(R* __restrict__ 
           Sc<R> v[4], d[4];
 #pragma unroll
           for (int q = 0; q < 4; ++q) {
-            v[q] = ldx<R, CX>(at(i + 32 * q, k));
-            d[q] = ldx<R, CX>(at(i + 32 * q, j));
+            v[q] = sc_ld<R, CX>(at(i + 32 * q, k));
+            d[q] = sc_ld<R, CX>(at(i + 32 * q, j));
           }
 #pragma unroll
           for (int q = 0; q < 4; ++q) acc = conj_mul_add<R, CX>(v[q], d[q], acc);
         }
-        for (; i < hi; i += 32) acc = conj_mul_add<R, CX>(ldx<R, CX>(at(i, k)), ldx<R, CX>(at(i, j)), acc);
+        for (; i < hi; i += 32) acc = conj_mul_add<R, CX>(sc_ld<R, CX>(at(i, k)), sc_ld<R, CX>(at(i, j)), acc);
       }
       acc.re = warp_sum(acc.re);
       if (CX) acc.im = warp_sum(acc.im);
@@ -476,10 +409,10 @@ __global__ void __launch_bounds__(CPQ_THREADS) colpiv_qr_kernel(R* __restrict__ 
         if (CX) acc.im += __ldcg(p + 1);
       }
       R* pu = at(k, j);
-      Sc<R> u = ldx<R, CX>(pu);
+      Sc<R> u = sc_ld<R, CX>(pu);
       Sc<R> d0;
       if (delayed) {
-        const Sc<R> tmp = mul_add<R, CX>(l, ldx<R, CX>(w.dot + W * j), u);
+        const Sc<R> tmp = mul_add<R, CX>(l, sc_ld<R, CX>(w.dot + W * j), u);
         d0 = scale<R, CX>(cadd<R, CX>(tmp, acc), -tau_inv);
         u = cadd<R, CX>(tmp, d0);
       } else {
@@ -487,8 +420,8 @@ __global__ void __launch_bounds__(CPQ_THREADS) colpiv_qr_kernel(R* __restrict__ 
         d0 = Sc<R>{-s.re, -s.im};
         u = cadd<R, CX>(u, d0);
       }
-      stx<R, CX>(pu, u);
-      stx<R, CX>(w.dot + W * j, d0);
+      sc_st<R, CX>(pu, u);
+      sc_st<R, CX>(w.dot + W * j, d0);
       const R nj = __ldcg(w.norm + j);
       w.norm[j] = sqrt(nj * nj - abs2<R, CX>(u));
     }
@@ -505,19 +438,6 @@ __global__ void __launch_bounds__(CPQ_THREADS) colpiv_qr_kernel(R* __restrict__ 
       if (CX) p[1] *= scale_fwd;
     }
   }
-}
-
-// dst(i, j) = src(i, j) over an m x n block (strided views in units of the scalar kind)
-template <class R, bool CX>
-__global__ void cpq_copy_kernel(R* __restrict__ dst, i64 drs, i64 dcs, const R* __restrict__ src, i64 srs, i64 scs, i64 m, i64 n) {
-  constexpr int W = CX ? 2 : 1;
-  const i64 e = (i64)blockIdx.x * blockDim.x + threadIdx.x;
-  if (e >= m * n) return;
-  const i64 i = e % m, j = e / m;
-  const R* q = src + W * (i * srs + j * scs);
-  R* p = dst + W * (i * drs + j * dcs);
-  p[0] = q[0];
-  if (CX) p[1] = q[1];
 }
 
 // Q_coeff[0, j] = Q_coeff[j % bs, j] = tau_j (factor.rs:374-376; the diagonal of every T block is its taus)
@@ -537,8 +457,6 @@ __global__ void cpq_tau_kernel(R* __restrict__ H, i64 rs, i64 cs, const R* __res
   }
 }
 
-inline unsigned cpq_blocks(i64 elems) { return (unsigned)((elems + 255) / 256); }
-
 inline void cpq_build_t(cudaStream_t st, View<const double> V, View<double> Tf, std::false_type) { householder_build_t<double>(st, V, Tf); }
 inline void cpq_build_t(cudaStream_t st, View<const float> V, View<float> Tf, std::false_type) { householder_build_t<float>(st, V, Tf); }
 inline void cpq_build_t(cudaStream_t st, View<const double> V, View<double> Tf, std::true_type) { householder_build_t_cx<double>(st, V, Tf); }
@@ -547,16 +465,15 @@ inline void cpq_build_t(cudaStream_t st, View<const float> V, View<float> Tf, st
 }  // namespace
 
 // In-place column-pivoted QR (views in element units of the scalar kind; complex: COMPLEX units on an R* base). H: block_size x
-// min(m, n). rs1: the caller's row stride is 1 (the reference's delayed-update condition). perm (host, n entries) receives perm_fwd.
-// Returns the transposition count.
+// min(m, n). rs1: the caller's row stride is 1 (the reference's delayed-update condition). trans (host, min(m, n) entries) receives
+// the column transpositions. Returns the transposition count.
 template <class R, bool CX>
-i64 colpiv_qr_in_place_t(cudaStream_t st, View<R> A, View<R> H, bool rs1, std::vector<long long>& perm) {
+i64 colpiv_qr_in_place_t(cudaStream_t st, View<R> A, View<R> H, bool rs1, std::vector<long long>& trans) {
   typedef std::integral_constant<bool, CX> Tag;
   constexpr int W = CX ? 2 : 1;
   const i64 m = A.nrows, n = A.ncols, size = std::min(m, n);
   FB_ASSERT(m < (i64)INT_MAX && n < (i64)INT_MAX, "column-pivoted QR: dimension too large");
-  perm.resize((size_t)n);
-  for (i64 j = 0; j < n; ++j) perm[(size_t)j] = j;
+  trans.assign((size_t)size, 0);
   if (size == 0) return 0;
   FB_ASSERT(H.nrows > 0 && H.ncols == size, "Q_coeff must be block_size x min(nrows, ncols) with block_size > 0");
 
@@ -567,9 +484,7 @@ i64 colpiv_qr_in_place_t(cudaStream_t st, View<R> A, View<R> H, bool rs1, std::v
   if (!compact) {
     work = (R*)ws_alloc((size_t)m * (size_t)n * W * sizeof(R));
     ld = m;
-    cpq_copy_kernel<R, CX><<<cpq_blocks(m * n), 256, 0, st>>>(work, 1, m, A.ptr, A.rs, A.cs, m, n);
-    FB_CUDA_CHECK(cudaGetLastError());
-    note_launch();
+    piv_copy_t<R, CX>(st, View<R>{work, m, n, 1, m}, cview(A));
   }
 
   const int sms = stream_sms(st);
@@ -602,14 +517,12 @@ i64 colpiv_qr_in_place_t(cudaStream_t st, View<R> A, View<R> H, bool rs1, std::v
     note_launch();
   }
   if (!compact) {
-    cpq_copy_kernel<R, CX><<<cpq_blocks(m * n), 256, 0, st>>>(A.ptr, A.rs, A.cs, work, 1, m, m, n);
-    FB_CUDA_CHECK(cudaGetLastError());
-    note_launch();
+    piv_copy_t<R, CX>(st, A, View<const R>{work, m, n, 1, m});
   }
 
   // T blocks (factor.rs:367-386)
   const i64 bs = H.nrows;
-  cpq_tau_kernel<R, CX><<<cpq_blocks(size), 256, 0, st>>>(H.ptr, H.rs, H.cs, w.tau, size, bs);
+  cpq_tau_kernel<R, CX><<<grid_1d(size), 256, 0, st>>>(H.ptr, H.rs, H.cs, w.tau, size, bs);
   FB_CUDA_CHECK(cudaGetLastError());
   note_launch();
   for (i64 j = 0; j < size; j += bs) {
@@ -625,11 +538,10 @@ i64 colpiv_qr_in_place_t(cudaStream_t st, View<R> A, View<R> H, bool rs1, std::v
   ws_free(buf);
   if (!compact) ws_free(work);
   i64 count = 0;
-  for (i64 k = 0; k < size; ++k)
-    if (hist[(size_t)k] != k) {
-      std::swap(perm[(size_t)k], perm[(size_t)hist[(size_t)k]]);
-      ++count;
-    }
+  for (i64 k = 0; k < size; ++k) {
+    trans[(size_t)k] = hist[(size_t)k];
+    count += hist[(size_t)k] != k;
+  }
   return count;
 }
 
@@ -650,33 +562,22 @@ FaerV0_24_ColPivQrStatus colpiv_qr_factor_entry(FaerV0_24_MatMut A, FaerV0_24_Ma
   FB_ASSERT(A.ncols == 0 || (perm_fwd.ptr != nullptr && perm_bwd.ptr != nullptr), "null permutation slice");
   cudaStream_t st = current_stream();
   const size_t es = (CX ? 2 : 1) * sizeof(R);
-  std::vector<long long> perm;
+  std::vector<long long> trans, fwd, bwd;
   i64 count = 0;
-  if (size == 0) {
-    perm.resize(A.ncols);
-    for (size_t j = 0; j < A.ncols; ++j) perm[j] = (long long)j;
-  } else {
+  if (size > 0) {
     StagedMat a(A.ptr, (i64)A.nrows, (i64)A.ncols, (i64)A.row_stride, (i64)A.col_stride, es, true, true, st);
     StagedMat q(Q_coeff.ptr, (i64)Q_coeff.nrows, (i64)Q_coeff.ncols, (i64)Q_coeff.row_stride, (i64)Q_coeff.col_stride, es, true, true, st);
-    count = colpiv_qr_in_place_t<R, CX>(st, a.view<R>(), q.view<R>(), A.row_stride == 1, perm);
+    count = colpiv_qr_in_place_t<R, CX>(st, a.view<R>(), q.view<R>(), A.row_stride == 1, trans);
     finish_all(st, {&a, &q});
   }
-  std::vector<long long> inv(perm.size());
-  for (size_t i = 0; i < perm.size(); ++i) inv[(size_t)perm[i]] = (long long)i;
-  write_perm(perm_fwd.ptr, perm, idx_bytes);
-  write_perm(perm_bwd.ptr, inv, idx_bytes);
+  perm_from_transpositions(A.ncols, trans, fwd, bwd);
+  write_perm(perm_fwd.ptr, fwd, idx_bytes);
+  write_perm(perm_bwd.ptr, bwd, idx_bytes);
   FaerV0_24_ColPivQrStatus out;
   memset(&out, 0, sizeof(out));
   out.tag = FaerV0_24_ColPivQrStatus_Ok;
   out.ok.transposition_count = (size_t)count;
   return out;
-}
-
-std::vector<long long> cpq_read_perm(FaerV0_24_SliceRef s, size_t n, int idx_bytes) {
-  FB_ASSERT(n == 0 || s.ptr != nullptr, "null permutation slice");
-  std::vector<long long> p = read_perm(s.ptr, n, idx_bytes);
-  for (size_t i = 0; i < n; ++i) FB_ASSERT(p[i] >= 0 && (size_t)p[i] < n, "invalid permutation entry");
-  return p;
 }
 
 // M (host or device) is staged once; `unpivoted` (an unpivoted QR entry point) runs on the device mirror, and rows [0, nrows) of
@@ -718,7 +619,7 @@ void cpq_staged(FaerV0_24_MatMut M, size_t nrows, const std::vector<long long>& 
                                                                                      size_t rhs_ncols, FaerV0_24_Par par) {              \
     /* StackReq::and(the unpivoted lstsq scratch, permute_rows_in_place_scratch::<I, T>(ncols, rhs_ncols)) */                              \
     const FaerV0_24_Layout a = libfaer_v0_23_qr_solve_lstsq_in_place_scratch_##SUF(nrows, ncols, block_size, rhs_ncols, par);             \
-    return cpq_and(a, ncols * rhs_ncols * (CX ? 2 : 1) * sizeof(R));                                                                      \
+    return layout_and(a, ncols * rhs_ncols * (CX ? 2 : 1) * sizeof(R));                                                                   \
   }                                                                                                                                       \
   FaerV0_24_Layout libfaer_v0_23_colpiv_qr_solve_in_place_scratch_##IT##_##SUF(size_t dim, size_t block_size, size_t rhs_ncols,           \
                                                                                FaerV0_24_Par par) {                                      \
@@ -727,7 +628,7 @@ void cpq_staged(FaerV0_24_MatMut M, size_t nrows, const std::vector<long long>& 
   FaerV0_24_Layout libfaer_v0_23_colpiv_qr_solve_transpose_in_place_scratch_##IT##_##SUF(size_t dim, size_t block_size,                   \
                                                                                          size_t rhs_ncols, FaerV0_24_Par par) {          \
     const FaerV0_24_Layout a = libfaer_v0_23_qr_solve_transpose_in_place_scratch_##SUF(dim, block_size, rhs_ncols, par);                  \
-    return cpq_and(a, dim * rhs_ncols * (CX ? 2 : 1) * sizeof(R));                                                                        \
+    return layout_and(a, dim * rhs_ncols * (CX ? 2 : 1) * sizeof(R));                                                                     \
   }                                                                                                                                       \
   void libfaer_v0_23_colpiv_qr_solve_lstsq_in_place_##IT##_##SUF(FaerV0_24_MatRef Q_basis, FaerV0_24_MatRef Q_coeff, FaerV0_24_MatRef R_, \
                                                                  FaerV0_24_Conj A_conj, FaerV0_24_SliceRef perm_fwd,                      \
@@ -736,7 +637,7 @@ void cpq_staged(FaerV0_24_MatMut M, size_t nrows, const std::vector<long long>& 
     FB_ENTRY();                                                                                                                           \
     (void)perm_fwd;                                                                                                                       \
     const size_t n = Q_basis.ncols;                                                                                                       \
-    const std::vector<long long> pb = cpq_read_perm(perm_bwd, n, BYTES);                                                                  \
+    const std::vector<long long> pb = read_perm_checked(perm_bwd, n, BYTES);                                                                  \
     /* the unpivoted lstsq, then rows ..size <- perm^-1 (solve.rs:66-79) */                                                             \
     cpq_staged<R, CX>(rhs, n, pb, false, false, [&](FaerV0_24_MatMut d) {                                                                 \
       libfaer_v0_23_qr_solve_lstsq_in_place_##SUF(Q_basis, Q_coeff, R_, A_conj, d, par, mem);                                            \
@@ -760,7 +661,7 @@ void cpq_staged(FaerV0_24_MatMut M, size_t nrows, const std::vector<long long>& 
     const size_t n = Q_basis.nrows;                                                                                                       \
     FB_ASSERT(Q_coeff.nrows > 0 && Q_basis.ncols == n && rhs.nrows == n && Q_coeff.ncols == n && R_.nrows == n && R_.ncols == n,        \
               "column-pivoted QR solve shape mismatch");                                                                                  \
-    const std::vector<long long> pf = cpq_read_perm(perm_fwd, n, BYTES);                                                                  \
+    const std::vector<long long> pf = read_perm_checked(perm_fwd, n, BYTES);                                                                  \
     /* rhs <- P rhs (solve.rs:180), then the unpivoted transpose solve */                                                               \
     cpq_staged<R, CX>(rhs, n, pf, false, true, [&](FaerV0_24_MatMut d) {                                                                  \
       libfaer_v0_23_qr_solve_transpose_in_place_##SUF(Q_basis, Q_coeff, R_, A_conj, d, par, mem);                                        \
@@ -780,7 +681,7 @@ void cpq_staged(FaerV0_24_MatMut M, size_t nrows, const std::vector<long long>& 
     (void)perm_fwd;                                                                                                                       \
     const size_t n = R_.ncols;                                                                                                            \
     FB_ASSERT(A.ncols == n, "column-pivoted QR reconstruct shape mismatch");                                                              \
-    const std::vector<long long> pb = cpq_read_perm(perm_bwd, n, BYTES);                                                                  \
+    const std::vector<long long> pb = read_perm_checked(perm_bwd, n, BYTES);                                                                  \
     /* Q R, then columns <- perm^-1 (reconstruct.rs:38-44) */                                                                          \
     cpq_staged<R, CX>(A, n, pb, true, false, [&](FaerV0_24_MatMut d) {                                                                    \
       libfaer_v0_23_qr_reconstruct_##SUF(d, Q_basis, Q_coeff, R_, par, mem);                                                             \
@@ -799,7 +700,7 @@ void cpq_staged(FaerV0_24_MatMut M, size_t nrows, const std::vector<long long>& 
     (void)perm_fwd;                                                                                                                       \
     const size_t n = Q_basis.ncols;                                                                                                       \
     FB_ASSERT(Q_coeff.nrows > 0 && A.nrows == n, "column-pivoted QR inverse shape mismatch");                                             \
-    const std::vector<long long> pb = cpq_read_perm(perm_bwd, n, BYTES);                                                                  \
+    const std::vector<long long> pb = read_perm_checked(perm_bwd, n, BYTES);                                                                  \
     /* R^-1 Q^H, then rows <- perm^-1 (inverse.rs:38-49) */                                                                            \
     cpq_staged<R, CX>(A, n, pb, false, false, [&](FaerV0_24_MatMut d) {                                                                   \
       libfaer_v0_23_qr_inverse_##SUF(d, Q_basis, Q_coeff, R_, par, mem);                                                                 \
@@ -811,15 +712,6 @@ void cpq_staged(FaerV0_24_MatMut M, size_t nrows, const std::vector<long long>& 
   }                                                                                                                 \
   FB_CPQ_FFI(SUF, R, CX, u32, 4)                                                                                    \
   FB_CPQ_FFI(SUF, R, CX, u64, 8)
-
-namespace {
-// StackReq::and: the second request placed after the first at its alignment (dyn-stack's rule for equal alignments)
-inline FaerV0_24_Layout cpq_and(FaerV0_24_Layout a, size_t b_bytes) {
-  const size_t al = a.align_bytes > 64 ? a.align_bytes : 64;
-  const size_t off = (a.len_bytes + 63) / 64 * 64;
-  return FaerV0_24_Layout{off + b_bytes, al};
-}
-}  // namespace
 
 extern "C" {
 FB_CPQ_DTYPE(f64, double, false)

@@ -1,5 +1,6 @@
-// Helpers shared by the translation units of the extern "C" boundary (ffi.cu, ffi_types.cu): scalar / permutation arguments that may
-// live on the host or on the device, and the end-of-call sequence of the staged matrices.
+// Helpers shared by the translation units of the extern "C" boundary (ffi.cu, ffi_types.cu and the pivoted factorizations): scalar /
+// permutation arguments that may live on the host or on the device, the end-of-call sequence of the staged matrices, and the
+// permutations and scratch layouts the pivoted families return.
 #pragma once
 #include "../../include/faer_b200.h"
 #include "runtime.cuh"
@@ -7,6 +8,7 @@
 #include <cstdint>
 #include <cstring>
 #include <initializer_list>
+#include <utility>
 #include <vector>
 
 namespace fb {
@@ -61,6 +63,30 @@ static inline void write_perm(void* dst, const std::vector<long long>& v, int id
   }
   if (is_device_pointer(dst)) FB_CUDA_CHECK(cudaMemcpy(dst, buf.data(), buf.size(), cudaMemcpyHostToDevice));
   else memcpy(dst, buf.data(), buf.size());
+}
+// a permutation of `n` entries that the caller hands in (PermRef::new_unchecked(fwd, bwd, min(fwd.len, bwd.len)) in the
+// reference; the length used is the matrix dimension, never the slice's `len`): a null slice or an entry outside [0, n) aborts
+static inline std::vector<long long> read_perm_checked(FaerV0_24_SliceRef s, size_t n, int idx_bytes) {
+  FB_ASSERT(n == 0 || s.ptr != nullptr, "null permutation slice");
+  std::vector<long long> p = read_perm(s.ptr, n, idx_bytes);
+  for (size_t i = 0; i < n; ++i) FB_ASSERT(p[i] >= 0 && (size_t)p[i] < n, "invalid permutation entry");
+  return p;
+}
+// fwd: the identity of `len` entries with the transpositions (i, t[i]) made in order; bwd: its inverse
+static inline void perm_from_transpositions(size_t len, const std::vector<long long>& t, std::vector<long long>& fwd,
+                                            std::vector<long long>& bwd) {
+  fwd.resize(len);
+  bwd.resize(len);
+  for (size_t i = 0; i < len; ++i) fwd[i] = (long long)i;
+  for (size_t i = 0; i < t.size(); ++i) std::swap(fwd[i], fwd[(size_t)t[i]]);
+  for (size_t i = 0; i < len; ++i) bwd[(size_t)fwd[i]] = (long long)i;
+}
+
+// StackReq::and: the second request placed after the first at its alignment (dyn-stack's rule for equal alignments)
+static inline FaerV0_24_Layout layout_and(FaerV0_24_Layout a, size_t b_bytes) {
+  const size_t al = a.align_bytes > 64 ? a.align_bytes : 64;
+  const size_t off = (a.len_bytes + 63) / 64 * 64;
+  return FaerV0_24_Layout{off + b_bytes, al};
 }
 
 }  // namespace fb

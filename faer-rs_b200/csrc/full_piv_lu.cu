@@ -28,13 +28,14 @@
 #include <climits>
 #include <cstdint>
 #include <cstdlib>
-#include <type_traits>
 #include <vector>
 
 #include "ffi_common.cuh"
 #include "panel_common.cuh"
+#include "piv_common.cuh"
 #include "pivot_record.cuh"
 #include "runtime.cuh"
+#include "scalar.cuh"
 #include "tensor_ops.cuh"
 
 namespace fb {
@@ -46,94 +47,23 @@ constexpr int FPL_WARPS = FPL_THREADS / 32;
 constexpr int FPL_TR = 128;  // rows of a trailing tile: 4 per lane
 constexpr int FPL_TC = 8;    // columns of a trailing tile
 
-// unfused arithmetic where the reference's scalar code rounds every operation
-__device__ __forceinline__ double fpl_mul(double a, double b) { return __dmul_rn(a, b); }
-__device__ __forceinline__ float fpl_mul(float a, float b) { return __fmul_rn(a, b); }
-__device__ __forceinline__ double fpl_add(double a, double b) { return __dadd_rn(a, b); }
-__device__ __forceinline__ float fpl_add(float a, float b) { return __fadd_rn(a, b); }
-__device__ __forceinline__ double fpl_sub(double a, double b) { return __dsub_rn(a, b); }
-__device__ __forceinline__ float fpl_sub(float a, float b) { return __fsub_rn(a, b); }
-
-// a scalar of the kind: (re, im), im == 0 for the real types
-template <class R>
-struct Fs {
-  R re, im;
-};
+// scalar.cuh's sc_ld / sc_st, except that a c64 element moves as one 16-byte access
 template <class R, bool CX>
-__device__ __forceinline__ Fs<R> fld(const R* p) {
+__device__ __forceinline__ Sc<R> fld(const R* p) {
   if (CX && sizeof(R) == 8) {  // one 16-byte access per c64 element (the working matrix is 16-byte aligned)
     const double2 v = __ldcg(reinterpret_cast<const double2*>(p));
-    return Fs<R>{(R)v.x, (R)v.y};
+    return Sc<R>{(R)v.x, (R)v.y};
   }
-  return Fs<R>{__ldcg(p), CX ? __ldcg(p + 1) : R(0)};
+  return Sc<R>{__ldcg(p), CX ? __ldcg(p + 1) : R(0)};
 }
 template <class R, bool CX>
-__device__ __forceinline__ void fst(R* p, Fs<R> v) {
+__device__ __forceinline__ void fst(R* p, Sc<R> v) {
   if (CX && sizeof(R) == 8) {
     *reinterpret_cast<double2*>(p) = make_double2((double)v.re, (double)v.im);
     return;
   }
   p[0] = v.re;
   if (CX) p[1] = v.im;
-}
-// a * b, each product and sum rounded (the reference's scalar `*=`)
-template <class R, bool CX>
-__device__ __forceinline__ Fs<R> fmul(Fs<R> a, Fs<R> b) {
-  if (!CX) return Fs<R>{fpl_mul(a.re, b.re), R(0)};
-  return Fs<R>{fpl_sub(fpl_mul(a.re, b.re), fpl_mul(a.im, b.im)), fpl_add(fpl_mul(a.re, b.im), fpl_mul(a.im, b.re))};
-}
-// acc + a * b as FMAs (the update's mul_add)
-template <class R, bool CX>
-__device__ __forceinline__ Fs<R> fmadd(Fs<R> a, Fs<R> b, Fs<R> acc) {
-  acc.re = fma(a.re, b.re, acc.re);
-  if (CX) {
-    acc.re = fma(-a.im, b.im, acc.re);
-    acc.im = fma(a.re, b.im, acc.im);
-    acc.im = fma(a.im, b.re, acc.im);
-  }
-  return acc;
-}
-// abs1: |re| + |im|
-template <class R, bool CX>
-__device__ __forceinline__ R fabs1(Fs<R> a) {
-  return CX ? fpl_add(fabs(a.re), fabs(a.im)) : fabs(a.re);
-}
-
-template <class R>
-struct FplLim;
-template <>
-struct FplLim<double> {
-  __device__ static double sml() { return 0x1p-511; }  // sqrt_min_positive
-  __device__ static double big() { return 0x1p511; }   // sqrt_max_positive
-};
-template <>
-struct FplLim<float> {
-  __device__ static float sml() { return 0x1p-63f; }
-  __device__ static float big() { return 0x1p63f; }
-};
-
-// recip: 1 / x for the real types; faer's recip_impl (faer-traits/src/lib.rs:353-383) for the complex ones
-template <class R, bool CX>
-__device__ __forceinline__ Fs<R> frecip(Fs<R> x) {
-  if (!CX) return Fs<R>{R(1) / x.re, R(0)};
-  const R re = x.re, im = x.im;
-  if (re != re || im != im) return Fs<R>{re + im, re + im};  // NaN
-  if (re == R(0) && im == R(0)) return Fs<R>{TLim<R>::inf(), TLim<R>::inf()};
-  if (!isfinite(re) || !isfinite(im)) return Fs<R>{R(0), R(0)};
-  const R sml = FplLim<R>::sml(), big = FplLim<R>::big();
-  const R ra = fabs(re), ia = fabs(im);
-  if (ra > big || ia > big) {
-    const R a = fpl_mul(re, sml), b = fpl_mul(im, sml);
-    const R inv = R(1) / fpl_add(fpl_mul(a, a), fpl_mul(b, b));
-    return Fs<R>{fpl_mul(fpl_mul(a, inv), sml), fpl_mul(fpl_mul(-b, inv), sml)};
-  }
-  if (ra > R(1) || ia > R(1)) {
-    const R inv = R(1) / fpl_add(fpl_mul(re, re), fpl_mul(im, im));
-    return Fs<R>{fpl_mul(re, inv), fpl_mul(-im, inv)};
-  }
-  const R a = fpl_mul(re, big), b = fpl_mul(im, big);
-  const R inv = R(1) / fpl_add(fpl_mul(a, a), fpl_mul(b, b));
-  return Fs<R>{fpl_mul(fpl_mul(a, inv), big), fpl_mul(fpl_mul(-b, inv), big)};
 }
 
 // per-CTA argmax record (pivot_record.cuh): the score and the column-major index i + j * m in X
@@ -172,7 +102,7 @@ __global__ void __launch_bounds__(FPL_THREADS) full_piv_lu_kernel(R* __restrict_
 
   // One pass over X[k0.., k0..] in tiles of FPL_TR x FPL_TC; with `upd`, x -= l_i u_j first (l, u from the workspace copies,
   // the side `tr` selects scaled by inv). Publishes this CTA's first maximum of abs1 to w.rec.
-  auto pass = [&](int k0, bool upd, Fs<R> inv) {
+  auto pass = [&](int k0, bool upd, Sc<R> inv) {
     R bv = R(0);
     long long bi = LLONG_MAX;
     const i64 nr = m - k0, nc = n - k0;
@@ -180,23 +110,23 @@ __global__ void __launch_bounds__(FPL_THREADS) full_piv_lu_kernel(R* __restrict_
     for (i64 t = gw; t < tiles_r * tiles_c; t += warps) {
       const i64 i0 = k0 + (t % tiles_r) * FPL_TR + lane;
       const i64 j0 = k0 + (t / tiles_r) * FPL_TC, j1 = min((i64)n, j0 + FPL_TC);
-      Fs<R> l[4];
+      Sc<R> l[4];
 #pragma unroll
       for (int q = 0; q < 4; ++q) {
-        l[q] = Fs<R>{R(0), R(0)};
+        l[q] = Sc<R>{R(0), R(0)};
         const i64 i = i0 + 32 * q;
         if (upd && i < m) {
           l[q] = fld<R, CX>(w.col + W * i);
-          if (!tr) l[q] = fmul<R, CX>(l[q], inv);
+          if (!tr) l[q] = cmul_rn<R, CX>(l[q], inv);
         }
       }
       // JB columns at a time: all their loads are issued before the first use (4 JB accesses in flight per lane)
       for (i64 jb = j0; jb < j1; jb += FPL_JB) {
-        Fs<R> u[FPL_JB], x[FPL_JB][4];
+        Sc<R> u[FPL_JB], x[FPL_JB][4];
         R* base = at(i0, jb);  // the 4 JB accesses of a lane are immediate offsets of one address
 #pragma unroll
         for (int c = 0; c < FPL_JB; ++c) {
-          u[c] = Fs<R>{R(0), R(0)};
+          u[c] = Sc<R>{R(0), R(0)};
           if (jb + c < j1) {
             if (upd) u[c] = fld<R, CX>(w.row + W * (jb + c));
 #pragma unroll
@@ -208,19 +138,19 @@ __global__ void __launch_bounds__(FPL_THREADS) full_piv_lu_kernel(R* __restrict_
         for (int c = 0; c < FPL_JB; ++c) {
           const i64 j = jb + c;
           if (j >= j1) continue;
-          if (upd && tr) u[c] = fmul<R, CX>(u[c], inv);
-          const Fs<R> nu{-u[c].re, -u[c].im};
+          if (upd && tr) u[c] = cmul_rn<R, CX>(u[c], inv);
+          const Sc<R> nu{-u[c].re, -u[c].im};
 #pragma unroll
           for (int q = 0; q < 4; ++q) {
             const i64 i = i0 + 32 * q;
             if (i < m) {
               if (upd) {
-                x[c][q] = fmadd<R, CX>(l[q], nu, x[c][q]);
+                x[c][q] = mul_add<R, CX>(l[q], nu, x[c][q]);
                 fst<R, CX>(base + W * (c * ld + 32 * q), x[c][q]);
               }
-              const R s = fabs1<R, CX>(x[c][q]);
+              const R s = abs1_rn<R, CX>(x[c][q]);
               const long long ix = i + j * (i64)m;
-              if (fpl_better(s, ix, bv, bi)) {
+              if (better(s, ix, bv, bi)) {
                 bv = s;
                 bi = ix;
               }
@@ -229,24 +159,10 @@ __global__ void __launch_bounds__(FPL_THREADS) full_piv_lu_kernel(R* __restrict_
         }
       }
     }
-    fpl_warp_argmax(bv, bi);
-    if (lane == 0) {
-      s_pv[warp] = bv;
-      s_pi[warp] = bi;
-    }
-    __syncthreads();
-    if (tid == 0) {
-      for (int q = 1; q < FPL_WARPS; ++q)
-        if (fpl_better(s_pv[q], s_pi[q], bv, bi)) {
-          bv = s_pv[q];
-          bi = s_pi[q];
-        }
-      w.rec[blockIdx.x].score = bv;
-      w.rec[blockIdx.x].idx = bi;
-    }
+    cta_publish<FPL_WARPS>(w.rec, bv, bi, s_pv, s_pi);
   };
 
-  pass(0, false, Fs<R>{R(0), R(0)});  // best_in_matrix(A), factor.rs:337
+  pass(0, false, Sc<R>{R(0), R(0)});  // best_in_matrix(A), factor.rs:337
   barrier();
 
   for (int k = 0; k < size; ++k) {
@@ -266,7 +182,7 @@ __global__ void __launch_bounds__(FPL_THREADS) full_piv_lu_kernel(R* __restrict_
         }
 #pragma unroll
         for (int u = 0; u < 4; ++u)
-          if (fpl_better(vs[u], is[u], v, ix)) {
+          if (better(vs[u], is[u], v, ix)) {
             v = vs[u];
             ix = is[u];
           }
@@ -292,9 +208,9 @@ __global__ void __launch_bounds__(FPL_THREADS) full_piv_lu_kernel(R* __restrict_
     // ---- S: swap rows k / r and columns k / c (factor.rs:349-358), copy the pivot column and row ----
     for (i64 i = gt; i < m; i += T) {  // column swap over the rows other than k and r
       if (i == k || i == r) continue;
-      Fs<R> v;
+      Sc<R> v;
       if (c != k) {
-        const Fs<R> a = fld<R, CX>(at(i, k)), b = fld<R, CX>(at(i, c));
+        const Sc<R> a = fld<R, CX>(at(i, k)), b = fld<R, CX>(at(i, c));
         fst<R, CX>(at(i, k), b);
         fst<R, CX>(at(i, c), a);
         v = b;
@@ -306,9 +222,9 @@ __global__ void __launch_bounds__(FPL_THREADS) full_piv_lu_kernel(R* __restrict_
     }
     for (i64 j = gt; j < n; j += T) {  // row swap over the columns other than k and c
       if (j == k || j == c) continue;
-      Fs<R> v;
+      Sc<R> v;
       if (r != k) {
-        const Fs<R> a = fld<R, CX>(at(k, j)), b = fld<R, CX>(at(r, j));
+        const Sc<R> a = fld<R, CX>(at(k, j)), b = fld<R, CX>(at(r, j));
         fst<R, CX>(at(k, j), b);
         fst<R, CX>(at(r, j), a);
         v = b;
@@ -320,7 +236,7 @@ __global__ void __launch_bounds__(FPL_THREADS) full_piv_lu_kernel(R* __restrict_
     }
     if (leader) {
       // the corner rows {k, r} x columns {k, c}: new(i, j) = old(swap_r(i), swap_c(j))
-      const Fs<R> o_kk = fld<R, CX>(at(k, k)), o_kc = fld<R, CX>(at(k, c)), o_rk = fld<R, CX>(at(r, k)), o_rc = fld<R, CX>(at(r, c));
+      const Sc<R> o_kk = fld<R, CX>(at(k, k)), o_kc = fld<R, CX>(at(k, c)), o_rk = fld<R, CX>(at(r, k)), o_rc = fld<R, CX>(at(r, c));
       fst<R, CX>(at(k, k), o_rc);
       fst<R, CX>(w.col + W * k, o_rc);  // the pivot
       if (c != k) {
@@ -338,54 +254,16 @@ __global__ void __launch_bounds__(FPL_THREADS) full_piv_lu_kernel(R* __restrict_
     barrier();
 
     // ---- U: scaled side (factor.rs:359-368), then the rank-one update fused with the next search (369-430) ----
-    const Fs<R> inv = frecip<R, CX>(fld<R, CX>(w.col + W * k));
+    const Sc<R> inv = recip_rn<R, CX>(fld<R, CX>(w.col + W * k));
     if (!tr) {
-      for (i64 i = k + 1 + gt; i < m; i += T) fst<R, CX>(at(i, k), fmul<R, CX>(fld<R, CX>(w.col + W * i), inv));
+      for (i64 i = k + 1 + gt; i < m; i += T) fst<R, CX>(at(i, k), cmul_rn<R, CX>(fld<R, CX>(w.col + W * i), inv));
     } else {
-      for (i64 j = k + 1 + gt; j < n; j += T) fst<R, CX>(at(k, j), fmul<R, CX>(fld<R, CX>(w.row + W * j), inv));
+      for (i64 j = k + 1 + gt; j < n; j += T) fst<R, CX>(at(k, j), cmul_rn<R, CX>(fld<R, CX>(w.row + W * j), inv));
     }
     if (k + 1 == size) break;
     pass(k + 1, true, inv);
     barrier();
   }
-}
-
-// dst(i, j) = src(i, j) over an m x n block (strided views in units of the scalar kind)
-template <class R, bool CX>
-__global__ void fpl_copy_kernel(R* __restrict__ dst, i64 drs, i64 dcs, const R* __restrict__ src, i64 srs, i64 scs, i64 m, i64 n) {
-  constexpr int W = CX ? 2 : 1;
-  const i64 e = (i64)blockIdx.x * blockDim.x + threadIdx.x;
-  if (e >= m * n) return;
-  const i64 i = e % m, j = e / m;
-  const R* q = src + W * (i * srs + j * scs);
-  R* p = dst + W * (i * drs + j * dcs);
-  p[0] = q[0];
-  if (CX) p[1] = q[1];
-}
-
-inline unsigned fpl_blocks(i64 elems) { return (unsigned)((elems + 255) / 256); }
-
-// ---- the building blocks by scalar kind ----
-inline void fpl_lower(cudaStream_t st, VCD t, bool unit, bool, VD rhs, std::false_type) { solve_lower_triangular_in_place_f64(st, t, unit, rhs); }
-inline void fpl_lower(cudaStream_t st, VCF t, bool unit, bool, VF rhs, std::false_type) { solve_lower_triangular_in_place_f32(st, t, unit, rhs); }
-inline void fpl_lower(cudaStream_t st, VCD t, bool unit, bool conj, VD rhs, std::true_type) { solve_lower_triangular_in_place_c64(st, t, unit, conj, rhs); }
-inline void fpl_lower(cudaStream_t st, VCF t, bool unit, bool conj, VF rhs, std::true_type) { solve_lower_triangular_in_place_c32(st, t, unit, conj, rhs); }
-inline void fpl_upper(cudaStream_t st, VCD t, bool unit, bool, VD rhs, std::false_type) { solve_upper_triangular_in_place_f64(st, t, unit, rhs); }
-inline void fpl_upper(cudaStream_t st, VCF t, bool unit, bool, VF rhs, std::false_type) { solve_upper_triangular_in_place_f32(st, t, unit, rhs); }
-inline void fpl_upper(cudaStream_t st, VCD t, bool unit, bool conj, VD rhs, std::true_type) { solve_upper_triangular_in_place_c64(st, t, unit, conj, rhs); }
-inline void fpl_upper(cudaStream_t st, VCF t, bool unit, bool conj, VF rhs, std::true_type) { solve_upper_triangular_in_place_c32(st, t, unit, conj, rhs); }
-// dst = lhs * rhs (Replace, alpha = 1) with the given block structures
-inline void fpl_gemm(cudaStream_t st, VD dst, VCD a, int as, VCD b, int bs, std::false_type) { gemm_f64(st, dst, RECT, 0, a, as, b, bs, 1.0); }
-inline void fpl_gemm(cudaStream_t st, VF dst, VCF a, int as, VCF b, int bs, std::false_type) { gemm_f32(st, dst, RECT, 0, a, as, b, bs, 1.0f); }
-inline void fpl_gemm(cudaStream_t st, VD dst, VCD a, int as, VCD b, int bs, std::true_type) {
-  gemm_c64(st, dst, RECT, 0, a, as, false, b, bs, false, 1.0, 0.0);
-}
-inline void fpl_gemm(cudaStream_t st, VF dst, VCF a, int as, VCF b, int bs, std::true_type) {
-  gemm_c32(st, dst, RECT, 0, a, as, false, b, bs, false, 1.0f, 0.0f);
-}
-template <class R, bool CX>
-View<R> fpl_sub(View<R> v, i64 i, i64 j, i64 m, i64 n) {
-  return View<R>{v.ptr + (CX ? 2 : 1) * (i * v.rs + j * v.cs), m, n, v.rs, v.cs};
 }
 
 // In-place full-pivoting LU (views in element units of the scalar kind; complex: COMPLEX units on an R* base). transpose: factor
@@ -408,9 +286,7 @@ i64 full_piv_lu_in_place_t(cudaStream_t st, View<R> A, bool transpose, std::vect
   if (!compact) {
     work = (R*)ws_alloc((size_t)m * (size_t)n * W * sizeof(R));
     ld = m;
-    fpl_copy_kernel<R, CX><<<fpl_blocks(m * n), 256, 0, st>>>(work, 1, m, V.ptr, V.rs, V.cs, m, n);
-    FB_CUDA_CHECK(cudaGetLastError());
-    note_launch();
+    piv_copy_t<R, CX>(st, View<R>{work, m, n, 1, m}, cview(V));
   }
 
   const int sms = stream_sms(st);
@@ -438,9 +314,7 @@ i64 full_piv_lu_in_place_t(cudaStream_t st, View<R> A, bool transpose, std::vect
     note_launch();
   }
   if (!compact) {
-    fpl_copy_kernel<R, CX><<<fpl_blocks(m * n), 256, 0, st>>>(V.ptr, V.rs, V.cs, work, 1, m, m, n);
-    FB_CUDA_CHECK(cudaGetLastError());
-    note_launch();
+    piv_copy_t<R, CX>(st, V, View<const R>{work, m, n, 1, m});
   }
   std::vector<int> hist((size_t)(2 * size));
   FB_CUDA_CHECK(cudaMemcpyAsync(hist.data(), w.hist, b_hist, cudaMemcpyDeviceToHost, st));
@@ -461,19 +335,18 @@ i64 full_piv_lu_in_place_t(cudaStream_t st, View<R> A, bool transpose, std::vect
 template <class R, bool CX>
 void full_piv_lu_solve_t(cudaStream_t st, View<const R> L, View<const R> U, const long long* row_fwd, const long long* row_bwd,
                          const long long* col_fwd, const long long* col_bwd, bool conj, bool transpose, View<R> rhs) {
-  typedef std::integral_constant<bool, CX> Tag;
   const i64 n = L.nrows;
   FB_ASSERT(L.ncols == n && U.nrows == n && U.ncols == n && rhs.nrows == n, "full-pivoting LU solve shape mismatch");
   if (n == 0 || rhs.ncols == 0) return;
   if (!transpose) {
     permute_rows_t<R, CX>(st, rhs, row_fwd);
-    fpl_lower(st, L, true, conj, rhs, Tag());
-    fpl_upper(st, U, false, conj, rhs, Tag());
+    solve_lower_t<R, CX>(st, L, true, conj, rhs);
+    solve_upper_t<R, CX>(st, U, false, conj, rhs);
     permute_rows_t<R, CX>(st, rhs, col_bwd);
   } else {
     permute_rows_t<R, CX>(st, rhs, col_fwd);
-    fpl_lower(st, U.t(), false, conj, rhs, Tag());
-    fpl_upper(st, L.t(), true, conj, rhs, Tag());
+    solve_lower_t<R, CX>(st, U.t(), false, conj, rhs);
+    solve_upper_t<R, CX>(st, L.t(), true, conj, rhs);
     permute_rows_t<R, CX>(st, rhs, row_bwd);
   }
 }
@@ -482,17 +355,20 @@ void full_piv_lu_solve_t(cudaStream_t st, View<const R> L, View<const R> U, cons
 template <class R, bool CX>
 void full_piv_lu_reconstruct_t(cudaStream_t st, View<R> out, View<const R> L, View<const R> U, const long long* row_bwd,
                                const long long* col_bwd) {
-  typedef std::integral_constant<bool, CX> Tag;
   constexpr int W = CX ? 2 : 1;
   const i64 m = L.nrows, n = U.ncols, size = std::min(m, n);
   FB_ASSERT(out.nrows == m && out.ncols == n && L.ncols >= size && U.nrows >= size, "full-pivoting LU reconstruct shape mismatch");
   if (m == 0 || n == 0) return;
   R* buf = (R*)ws_alloc((size_t)m * (size_t)n * W * sizeof(R));
   const View<R> tmp{buf, m, n, 1, m};
-  const View<const R> Ls = fpl_sub<const R, CX>(L, 0, 0, size, size), Us = fpl_sub<const R, CX>(U, 0, 0, size, size);
-  fpl_gemm(st, fpl_sub<R, CX>(tmp, 0, 0, size, size), Ls, UNIT_LOWER, Us, TRI_UPPER, Tag());
-  if (m > n) fpl_gemm(st, fpl_sub<R, CX>(tmp, size, 0, m - size, size), fpl_sub<const R, CX>(L, size, 0, m - size, size), RECT, Us, TRI_UPPER, Tag());
-  if (m < n) fpl_gemm(st, fpl_sub<R, CX>(tmp, 0, size, size, n - size), Ls, UNIT_LOWER, fpl_sub<const R, CX>(U, 0, size, size, n - size), RECT, Tag());
+  const View<const R> Ls = sub_t<R, CX>(L, 0, 0, size, size), Us = sub_t<R, CX>(U, 0, 0, size, size);
+  gemm_t<R, CX>(st, sub_t<R, CX>(tmp, 0, 0, size, size), RECT, 0, Ls, UNIT_LOWER, false, Us, TRI_UPPER, false, R(1));
+  if (m > n)
+    gemm_t<R, CX>(st, sub_t<R, CX>(tmp, size, 0, m - size, size), RECT, 0, sub_t<R, CX>(L, size, 0, m - size, size), RECT, false, Us,
+                  TRI_UPPER, false, R(1));
+  if (m < n)
+    gemm_t<R, CX>(st, sub_t<R, CX>(tmp, 0, size, size, n - size), RECT, 0, Ls, UNIT_LOWER, false, sub_t<R, CX>(U, 0, size, size, n - size),
+                  RECT, false, R(1));
   gather_2d_t<R, CX>(st, out, View<const R>{buf, m, n, 1, m}, row_bwd, col_bwd);
   ws_free(buf);
 }
@@ -502,7 +378,6 @@ void full_piv_lu_reconstruct_t(cudaStream_t st, View<R> out, View<const R> L, Vi
 template <class R, bool CX>
 void full_piv_lu_inverse_t(cudaStream_t st, View<R> out, View<const R> L, View<const R> U, const long long* row_bwd,
                            const long long* col_bwd) {
-  typedef std::integral_constant<bool, CX> Tag;
   constexpr int W = CX ? 2 : 1;
   const i64 n = L.nrows;
   FB_ASSERT(L.ncols == n && U.nrows == n && U.ncols == n && out.nrows == n && out.ncols == n, "full-pivoting LU inverse shape mismatch");
@@ -511,7 +386,7 @@ void full_piv_lu_inverse_t(cudaStream_t st, View<R> out, View<const R> L, View<c
   inverse_triangular_t<R, CX>(st, out, U, false, false);
   R* buf = (R*)ws_alloc((size_t)n * (size_t)n * W * sizeof(R));
   const View<const R> o{out.ptr, n, n, out.rs, out.cs};
-  fpl_gemm(st, View<R>{buf, n, n, 1, n}, o, TRI_UPPER, o, UNIT_LOWER, Tag());
+  gemm_t<R, CX>(st, View<R>{buf, n, n, 1, n}, RECT, 0, o, TRI_UPPER, false, o, UNIT_LOWER, false, R(1));
   gather_2d_t<R, CX>(st, out, View<const R>{buf, n, n, 1, n}, col_bwd, row_bwd);
   ws_free(buf);
 }
@@ -544,16 +419,9 @@ FaerV0_24_FullPivLuStatus full_piv_lu_factor_entry(FaerV0_24_MatMut A, FaerV0_24
     finish_all(st, {&a});
   }
   // factor.rs:511-528: the transpositions applied in order to the identity, and the inverses
-  auto perms = [](size_t len, const std::vector<long long>& t, std::vector<long long>& fwd, std::vector<long long>& bwd) {
-    fwd.resize(len);
-    bwd.resize(len);
-    for (size_t i = 0; i < len; ++i) fwd[i] = (long long)i;
-    for (size_t i = 0; i < t.size(); ++i) std::swap(fwd[i], fwd[(size_t)t[i]]);
-    for (size_t i = 0; i < len; ++i) bwd[(size_t)fwd[i]] = (long long)i;
-  };
   std::vector<long long> rf, rb, cf, cb;
-  perms(m, rt, rf, rb);
-  perms(n, ct, cf, cb);
+  perm_from_transpositions(m, rt, rf, rb);
+  perm_from_transpositions(n, ct, cf, cb);
   write_perm(row_fwd.ptr, rf, idx_bytes);
   write_perm(row_bwd.ptr, rb, idx_bytes);
   write_perm(col_fwd.ptr, cf, idx_bytes);
@@ -565,15 +433,6 @@ FaerV0_24_FullPivLuStatus full_piv_lu_factor_entry(FaerV0_24_MatMut A, FaerV0_24
   return out;
 }
 
-// a permutation of `n` entries (PermRef::new_unchecked(fwd, bwd, min(fwd.len, bwd.len)) in the reference; the length used here is
-// the matrix dimension, never the slices' `len`)
-std::vector<long long> fpl_read_perm(FaerV0_24_SliceRef s, size_t n, int idx_bytes) {
-  FB_ASSERT(n == 0 || s.ptr != nullptr, "null permutation slice");
-  std::vector<long long> p = read_perm(s.ptr, n, idx_bytes);
-  for (size_t i = 0; i < n; ++i) FB_ASSERT(p[i] >= 0 && (size_t)p[i] < n, "invalid permutation entry");
-  return p;
-}
-
 template <class R, bool CX>
 void full_piv_lu_solve_entry(FaerV0_24_MatRef L, FaerV0_24_MatRef U, FaerV0_24_Conj conj, FaerV0_24_SliceRef row_fwd,
                              FaerV0_24_SliceRef row_bwd, FaerV0_24_SliceRef col_fwd, FaerV0_24_SliceRef col_bwd, FaerV0_24_MatMut rhs,
@@ -583,8 +442,8 @@ void full_piv_lu_solve_entry(FaerV0_24_MatRef L, FaerV0_24_MatRef U, FaerV0_24_C
   FB_ASSERT(L.ncols == n && U.nrows == n && U.ncols == n && rhs.nrows == n, "full-pivoting LU solve shape mismatch");
   cudaStream_t st = current_stream();
   const size_t es = (CX ? 2 : 1) * sizeof(R);
-  const std::vector<long long> rf = fpl_read_perm(row_fwd, n, idx_bytes), rb = fpl_read_perm(row_bwd, n, idx_bytes);
-  const std::vector<long long> cf = fpl_read_perm(col_fwd, n, idx_bytes), cb = fpl_read_perm(col_bwd, n, idx_bytes);
+  const std::vector<long long> rf = read_perm_checked(row_fwd, n, idx_bytes), rb = read_perm_checked(row_bwd, n, idx_bytes);
+  const std::vector<long long> cf = read_perm_checked(col_fwd, n, idx_bytes), cb = read_perm_checked(col_bwd, n, idx_bytes);
   StagedMat l(L.ptr, (i64)n, (i64)n, (i64)L.row_stride, (i64)L.col_stride, es, true, false, st);
   StagedMat u(U.ptr, (i64)n, (i64)n, (i64)U.row_stride, (i64)U.col_stride, es, true, false, st);
   StagedMat r(rhs.ptr, (i64)rhs.nrows, (i64)rhs.ncols, (i64)rhs.row_stride, (i64)rhs.col_stride, es, true, true, st);
@@ -605,7 +464,7 @@ void full_piv_lu_recon_entry(FaerV0_24_MatMut A, FaerV0_24_MatRef L, FaerV0_24_M
               "full-pivoting LU reconstruct shape mismatch");
   cudaStream_t st = current_stream();
   const size_t es = (CX ? 2 : 1) * sizeof(R);
-  const std::vector<long long> rb = fpl_read_perm(row_bwd, m, idx_bytes), cb = fpl_read_perm(col_bwd, n, idx_bytes);
+  const std::vector<long long> rb = read_perm_checked(row_bwd, m, idx_bytes), cb = read_perm_checked(col_bwd, n, idx_bytes);
   StagedMat a(A.ptr, (i64)A.nrows, (i64)A.ncols, (i64)A.row_stride, (i64)A.col_stride, es, false, true, st);
   StagedMat l(L.ptr, (i64)L.nrows, (i64)L.ncols, (i64)L.row_stride, (i64)L.col_stride, es, true, false, st);
   StagedMat u(U.ptr, (i64)U.nrows, (i64)U.ncols, (i64)U.row_stride, (i64)U.col_stride, es, true, false, st);

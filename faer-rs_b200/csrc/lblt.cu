@@ -39,7 +39,7 @@
 //                       -> barrier, plus one barrier per extra candidate column. The scaled L columns of a pivot are written one
 //                       pivot later (the update reads them unscaled; row interchanges commute with the per-row scaling), which
 //                       keeps the writers and the readers of a pivot column in different phases. The trailing pass is tiled:
-//                       a warp owns 128 consecutive rows of one column. Records use pivot_record.cuh (full_piv_lu.cu's).
+//                       a warp owns 128 consecutive rows of one column. Records and their publish are pivot_record.cuh's.
 // Pivots and 2 x 2 flags stay on the device and are read back once, after the factorization.
 // Record sets: A (diagonal argmax), B (the first candidate column) and C. Further candidate columns of one decision (the second
 // test, the rook walk) alternate C, B, C, ... (lb_cand): every CTA reads a set after a barrier, and a CTA that leaves the barrier
@@ -53,7 +53,6 @@
 #include <algorithm>
 #include <climits>
 #include <cstring>
-#include <type_traits>
 #include <vector>
 
 #include "ffi_common.cuh"
@@ -61,6 +60,7 @@
 #include "piv_common.cuh"
 #include "pivot_record.cuh"
 #include "runtime.cuh"
+#include "scalar.cuh"
 #include "tensor_ops.cuh"
 
 namespace fb {
@@ -71,49 +71,6 @@ constexpr int LB_THREADS = 256;
 constexpr int LB_WARPS = LB_THREADS / 32;
 constexpr int LB_TR = 128;  // rows of a trailing tile of the right-looking kernel: 4 per lane
 
-// a scalar of the kind: (re, im), im == 0 for the real types
-template <class R>
-struct Cx {
-  R re, im;
-};
-template <class R, bool CX>
-__device__ __forceinline__ Cx<R> cld(const R* p) {
-  return Cx<R>{__ldcg(p), CX ? __ldcg(p + 1) : R(0)};
-}
-template <class R, bool CX>
-__device__ __forceinline__ void cst(R* p, Cx<R> v) {
-  p[0] = v.re;
-  if (CX) p[1] = v.im;
-}
-template <class R>
-__device__ __forceinline__ Cx<R> cconj(Cx<R> a) { return Cx<R>{a.re, -a.im}; }
-template <class R>
-__device__ __forceinline__ Cx<R> csub(Cx<R> a, Cx<R> b) { return Cx<R>{a.re - b.re, a.im - b.im}; }
-template <class R>
-__device__ __forceinline__ Cx<R> cscale(Cx<R> a, R s) { return Cx<R>{a.re * s, a.im * s}; }
-template <class R, bool CX>
-__device__ __forceinline__ Cx<R> cmul(Cx<R> a, Cx<R> b) {
-  if (!CX) return Cx<R>{a.re * b.re, R(0)};
-  return Cx<R>{a.re * b.re - a.im * b.im, a.re * b.im + a.im * b.re};
-}
-// acc - a * conj(b), as FMAs
-template <class R, bool CX>
-__device__ __forceinline__ Cx<R> cfms_conj(Cx<R> acc, Cx<R> a, Cx<R> b) {
-  acc.re = fma(-a.re, b.re, acc.re);
-  if (CX) {
-    acc.re = fma(-a.im, b.im, acc.re);
-    acc.im = fma(a.re, b.im, acc.im);
-    acc.im = fma(-a.im, b.re, acc.im);
-  }
-  return acc;
-}
-template <class R>
-__device__ __forceinline__ R cabs1(Cx<R> a) { return fabs(a.re) + fabs(a.im); }
-template <class R>
-__device__ __forceinline__ R cabs2(Cx<R> a) { return a.re * a.re + a.im * a.im; }
-template <class R, bool CX>
-__device__ __forceinline__ R cabs(Cx<R> a) { return CX ? hypot(a.re, a.im) : fabs(a.re); }
-
 // a pivot block whose scaling / update is pending: kind 0 none (also "nothing to do"), 1 a 1 x 1 pivot at column p, 2 a 2 x 2 pivot
 // at columns p, p + 1 (factor.rs:620-670 / 867-891 / 337-393)
 template <class R>
@@ -121,7 +78,7 @@ struct LbPiv {
   int kind, p;
   R dg, dinv;          // 1 x 1: Re a_pp, recip
   R d, d00, d11;       // 2 x 2
-  Cx<R> d10;
+  Sc<R> d10;
 };
 template <class R, bool CX>
 __device__ __forceinline__ LbPiv<R> lb_one(int p, R dg) {
@@ -133,7 +90,7 @@ __device__ __forceinline__ LbPiv<R> lb_one(int p, R dg) {
   return q;
 }
 template <class R, bool CX>
-__device__ __forceinline__ LbPiv<R> lb_two(int p, R a00, R a11, Cx<R> a10) {
+__device__ __forceinline__ LbPiv<R> lb_two(int p, R a00, R a11, Sc<R> a10) {
   LbPiv<R> q{};
   q.kind = 2;
   q.p = p;
@@ -148,7 +105,7 @@ __device__ __forceinline__ LbPiv<R> lb_two(int p, R a00, R a11, Cx<R> a10) {
 }
 // w0 = (x0 d11 - x1 d10) d, w1 = (x1 d00 - x0 conj(d10)) d
 template <class R, bool CX>
-__device__ __forceinline__ void lb_w(const LbPiv<R>& q, Cx<R> x0, Cx<R> x1, Cx<R>& w0, Cx<R>& w1) {
+__device__ __forceinline__ void lb_w(const LbPiv<R>& q, Sc<R> x0, Sc<R> x1, Sc<R>& w0, Sc<R>& w1) {
   w0 = cscale(csub(cscale(x0, q.d11), cmul<R, CX>(x1, q.d10)), q.d);
   w1 = cscale(csub(cscale(x1, q.d00), cmul<R, CX>(x0, cconj(q.d10))), q.d);
 }
@@ -165,22 +122,7 @@ struct LbWs {
 // this CTA's first maximum into rec[blockIdx.x] (every thread of the CTA calls it)
 template <class R>
 __device__ void lb_publish(FplRec<R>* rec, R v, long long i, R* s_v, long long* s_i) {
-  fpl_warp_argmax(v, i);
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  if (lane == 0) {
-    s_v[warp] = v;
-    s_i[warp] = i;
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    for (int q = 1; q < LB_WARPS; ++q)
-      if (fpl_better(s_v[q], s_i[q], v, i)) {
-        v = s_v[q];
-        i = s_i[q];
-      }
-    rec[blockIdx.x].score = v;
-    rec[blockIdx.x].idx = i;
-  }
+  cta_publish<LB_WARPS>(rec, v, i, s_v, s_i);
   __syncthreads();
 }
 // the same reduction of the grid's records in every CTA (after a grid barrier)
@@ -192,7 +134,7 @@ __device__ void lb_collect(const FplRec<R>* rec, R& v, long long& i, R* s_v, lon
     for (int b = threadIdx.x; b < (int)gridDim.x; b += 32) {
       const R v2 = __ldcg(&rec[b].score);
       const long long i2 = __ldcg(&rec[b].idx);
-      if (fpl_better(v2, i2, bv, bi)) {
+      if (better(v2, i2, bv, bi)) {
         bv = v2;
         bi = i2;
       }
@@ -227,30 +169,30 @@ __device__ void lb_swap(At at, Wa wa, bool with_w, int m, int i, int j, int nw, 
   for (i64 e = gt; e < na + nb + nc + nd; e += T) {
     if (e < na) {
       const i64 r = j + 1 + e;
-      const Cx<R> x = cld<R, CX>(at(r, i)), y = cld<R, CX>(at(r, j));
-      cst<R, CX>(at(r, i), y);
-      cst<R, CX>(at(r, j), x);
+      const Sc<R> x = sc_ld<R, CX>(at(r, i)), y = sc_ld<R, CX>(at(r, j));
+      sc_st<R, CX>(at(r, i), y);
+      sc_st<R, CX>(at(r, j), x);
     } else if (e < na + nb) {
       const i64 col = e - na;
-      const Cx<R> x = cld<R, CX>(at(i, col)), y = cld<R, CX>(at(j, col));
-      cst<R, CX>(at(i, col), y);
-      cst<R, CX>(at(j, col), x);
+      const Sc<R> x = sc_ld<R, CX>(at(i, col)), y = sc_ld<R, CX>(at(j, col));
+      sc_st<R, CX>(at(i, col), y);
+      sc_st<R, CX>(at(j, col), x);
     } else if (e < na + nb + nc) {
       const i64 t = i + 1 + (e - na - nb);
-      const Cx<R> x = cld<R, CX>(at(t, i)), y = cld<R, CX>(at(j, t));
-      cst<R, CX>(at(t, i), cconj(y));
-      cst<R, CX>(at(j, t), cconj(x));
+      const Sc<R> x = sc_ld<R, CX>(at(t, i)), y = sc_ld<R, CX>(at(j, t));
+      sc_st<R, CX>(at(t, i), cconj(y));
+      sc_st<R, CX>(at(j, t), cconj(x));
     } else {
       const i64 col = e - na - nb - nc;
-      const Cx<R> x = cld<R, CX>(wa(i, col)), y = cld<R, CX>(wa(j, col));
-      cst<R, CX>(wa(i, col), y);
-      cst<R, CX>(wa(j, col), x);
+      const Sc<R> x = sc_ld<R, CX>(wa(i, col)), y = sc_ld<R, CX>(wa(j, col));
+      sc_st<R, CX>(wa(i, col), y);
+      sc_st<R, CX>(wa(j, col), x);
     }
   }
   if (leader) {
     const R aii = __ldcg(at(i, i)), ajj = __ldcg(at(j, j));
-    cst<R, CX>(at(i, i), Cx<R>{ajj, R(0)});
-    cst<R, CX>(at(j, j), Cx<R>{aii, R(0)});
+    sc_st<R, CX>(at(i, i), Sc<R>{ajj, R(0)});
+    sc_st<R, CX>(at(j, j), Sc<R>{aii, R(0)});
     if (CX) {
       R* o = at(j, i);
       o[1] = -__ldcg(o + 1);
@@ -289,27 +231,27 @@ __global__ void __launch_bounds__(LB_THREADS, 1) lblt_panel_kernel(R* __restrict
     for (i64 r = gt; r < m; r += T) {
       if (r < c) continue;
       if (q.kind == 1) {
-        const Cx<R> l = cscale(cld<R, CX>(wa(r, q.p)), q.dinv);
-        cst<R, CX>(at(r, q.p), l);
-        cst<R, CX>(at(r, r), Cx<R>{__ldcg(at(r, r)) - q.dg * cabs2(l), R(0)});
+        const Sc<R> l = cscale(sc_ld<R, CX>(wa(r, q.p)), q.dinv);
+        sc_st<R, CX>(at(r, q.p), l);
+        sc_st<R, CX>(at(r, r), Sc<R>{__ldcg(at(r, r)) - q.dg * cabs2(l), R(0)});
       } else if (q.kind == 2) {
-        const Cx<R> x0 = cld<R, CX>(wa(r, q.p)), x1 = cld<R, CX>(wa(r, q.p + 1));
-        Cx<R> w0, w1;
+        const Sc<R> x0 = sc_ld<R, CX>(wa(r, q.p)), x1 = sc_ld<R, CX>(wa(r, q.p + 1));
+        Sc<R> w0, w1;
         lb_w<R, CX>(q, x0, x1, w0, w1);
-        const Cx<R> a = csub(csub(cld<R, CX>(at(r, r)), cmul<R, CX>(x0, cconj(w0))), cmul<R, CX>(x1, cconj(w1)));
-        cst<R, CX>(at(r, r), Cx<R>{a.re, R(0)});
-        cst<R, CX>(at(r, q.p), w0);
-        cst<R, CX>(at(r, q.p + 1), w1);
+        const Sc<R> a = csub(csub(sc_ld<R, CX>(at(r, r)), cmul<R, CX>(x0, cconj(w0))), cmul<R, CX>(x1, cconj(w1)));
+        sc_st<R, CX>(at(r, r), Sc<R>{a.re, R(0)});
+        sc_st<R, CX>(at(r, q.p), w0);
+        sc_st<R, CX>(at(r, q.p + 1), w1);
       }
       if (want) {
-        const R s = cabs1(cld<R, CX>(at(r, r)));
+        const R s = cabs1(sc_ld<R, CX>(at(r, r)));
         if (s > bv) {
           bv = s;
           bi = r;
         }
       }
     }
-    if (leader && q.kind == 2) cst<R, CX>(at(q.p + 1, q.p), Cx<R>{R(0), R(0)});
+    if (leader && q.kind == 2) sc_st<R, CX>(at(q.p + 1, q.p), Sc<R>{R(0), R(0)});
     if (want) lb_publish(recA, bv, bi, s_v, s_i);
   };
   // W[:, wc] <- column x of the updated trailing matrix, rows c.. (update_and_offdiag_argmax, factor.rs:461-489), and the
@@ -320,17 +262,17 @@ __global__ void __launch_bounds__(LB_THREADS, 1) lblt_panel_kernel(R* __restrict
     for (i64 r = gt; r < m; r += T) {
       if (r < c) continue;
       if (r == x) {
-        cst<R, CX>(wa(r, wc), Cx<R>{__ldcg(at(r, r)), R(0)});
+        sc_st<R, CX>(wa(r, wc), Sc<R>{__ldcg(at(r, r)), R(0)});
         continue;
       }
-      Cx<R> v = r < x ? cconj(cld<R, CX>(at(x, r))) : cld<R, CX>(at(r, x));
-      Cx<R> acc{R(0), R(0)};
+      Sc<R> v = r < x ? cconj(sc_ld<R, CX>(at(x, r))) : sc_ld<R, CX>(at(r, x));
+      Sc<R> acc{R(0), R(0)};
       for (int t = 0; t < c; ++t) {
-        const Cx<R> a = cld<R, CX>(at(r, t)), b = cld<R, CX>(wa(x, t));
+        const Sc<R> a = sc_ld<R, CX>(at(r, t)), b = sc_ld<R, CX>(wa(x, t));
         acc = cfms_conj<R, CX>(acc, a, b);  // acc -= Al[r, t] conj(Wl[x, t])
       }
-      v = Cx<R>{v.re + acc.re, v.im + acc.im};
-      cst<R, CX>(wa(r, wc), v);
+      v = Sc<R>{v.re + acc.re, v.im + acc.im};
+      sc_st<R, CX>(wa(r, wc), v);
       const R s = cabs1(v);
       if (s > bv) {
         bv = s;
@@ -341,7 +283,7 @@ __global__ void __launch_bounds__(LB_THREADS, 1) lblt_panel_kernel(R* __restrict
   };
   auto copy_col = [&](int c, int from, int to) {
     for (i64 r = gt; r < m; r += T)
-      if (r >= c) cst<R, CX>(wa(r, to), cld<R, CX>(wa(r, from)));
+      if (r >= c) sc_st<R, CX>(wa(r, to), sc_ld<R, CX>(wa(r, from)));
   };
 
   LbPiv<R> q{};
@@ -382,7 +324,7 @@ __global__ void __launch_bounds__(LB_THREADS, 1) lblt_panel_kernel(R* __restrict
           long long s;
           lb_collect(set, gr, s, s_v, s_i);
           if (s == LLONG_MAX) s = c;
-          if (cabs1(cld<R, CX>(at(i1, i1))) >= alpha * gr) {
+          if (cabs1(sc_ld<R, CX>(at(i1, i1))) >= alpha * gr) {
             npiv = 1;
             i0 = i1;
             i1 = -1;
@@ -423,9 +365,9 @@ __global__ void __launch_bounds__(LB_THREADS, 1) lblt_panel_kernel(R* __restrict
       if (i0 > i1) {
         for (i64 rr = gt; rr < m; rr += T) {
           if (rr < c) continue;
-          const Cx<R> x = cld<R, CX>(wa(rr, c)), y = cld<R, CX>(wa(rr, c + 1));
-          cst<R, CX>(wa(rr, c), y);
-          cst<R, CX>(wa(rr, c + 1), x);
+          const Sc<R> x = sc_ld<R, CX>(wa(rr, c)), y = sc_ld<R, CX>(wa(rr, c + 1));
+          sc_st<R, CX>(wa(rr, c), y);
+          sc_st<R, CX>(wa(rr, c + 1), x);
         }
         const int t = i0;
         i0 = i1;
@@ -452,13 +394,13 @@ __global__ void __launch_bounds__(LB_THREADS, 1) lblt_panel_kernel(R* __restrict
       q.kind = 0;
     } else if (npiv == 1) {
       q = lb_one<R, CX>(c, __ldcg(wa(c, c)));
-      if (leader) cst<R, CX>(sd(c), Cx<R>{R(0), R(0)});
+      if (leader) sc_st<R, CX>(sd(c), Sc<R>{R(0), R(0)});
     } else {
-      const Cx<R> a10 = cld<R, CX>(wa(c + 1, c));
+      const Sc<R> a10 = sc_ld<R, CX>(wa(c + 1, c));
       q = lb_two<R, CX>(c, __ldcg(wa(c, c)), __ldcg(wa(c + 1, c + 1)), a10);
       if (leader) {
-        cst<R, CX>(sd(c), a10);
-        cst<R, CX>(sd(c + 1), Cx<R>{R(0), R(0)});
+        sc_st<R, CX>(sd(c), a10);
+        sc_st<R, CX>(sd(c + 1), Sc<R>{R(0), R(0)});
       }
     }
     c += npiv;
@@ -497,15 +439,15 @@ __global__ void __launch_bounds__(LB_THREADS, 1) lblt_rl_kernel(R* __restrict__ 
     if (s.kind == 0) return;
     for (i64 r = s.p + s.kind + gt; r < m; r += T) {
       if (s.kind == 1) {
-        cst<R, CX>(at(r, s.p), cscale(cld<R, CX>(at(r, s.p)), s.dinv));
+        sc_st<R, CX>(at(r, s.p), cscale(sc_ld<R, CX>(at(r, s.p)), s.dinv));
       } else {
-        Cx<R> w0, w1;
-        lb_w<R, CX>(s, cld<R, CX>(at(r, s.p)), cld<R, CX>(at(r, s.p + 1)), w0, w1);
-        cst<R, CX>(at(r, s.p), w0);
-        cst<R, CX>(at(r, s.p + 1), w1);
+        Sc<R> w0, w1;
+        lb_w<R, CX>(s, sc_ld<R, CX>(at(r, s.p)), sc_ld<R, CX>(at(r, s.p + 1)), w0, w1);
+        sc_st<R, CX>(at(r, s.p), w0);
+        sc_st<R, CX>(at(r, s.p + 1), w1);
       }
     }
-    if (leader && s.kind == 2) cst<R, CX>(at(s.p + 1, s.p), Cx<R>{R(0), R(0)});
+    if (leader && s.kind == 2) sc_st<R, CX>(at(s.p + 1, s.p), Sc<R>{R(0), R(0)});
   };
   // The trailing lower triangle from column c: the update of pivot q (rank1_update / rank2_update, or Full's
   // rank_*_update_and_argmax with its diagonal update), the deferred columns of s, and the records: A = diagonal (abs1, Full:
@@ -522,56 +464,56 @@ __global__ void __launch_bounds__(LB_THREADS, 1) lblt_rl_kernel(R* __restrict__ 
       const i64 i0 = c + rb * LB_TR;
       if (i0 + LB_TR <= j) continue;  // above the diagonal
       if (!full_pass && !(diagonal ? (j >= i0) : (j == c))) continue;
-      Cx<R> w0{R(0), R(0)}, w1{R(0), R(0)};
+      Sc<R> w0{R(0), R(0)}, w1{R(0), R(0)};
       if (q.kind == 1) {
-        w0 = cscale(cld<R, CX>(at(j, q.p)), q.dinv);  // unblocked: w0 = L[j] d; Full: L[j] scaled
+        w0 = cscale(sc_ld<R, CX>(at(j, q.p)), q.dinv);  // unblocked: w0 = L[j] d; Full: L[j] scaled
       } else if (q.kind == 2) {
-        lb_w<R, CX>(q, cld<R, CX>(at(j, q.p)), cld<R, CX>(at(j, q.p + 1)), w0, w1);
+        lb_w<R, CX>(q, sc_ld<R, CX>(at(j, q.p)), sc_ld<R, CX>(at(j, q.p + 1)), w0, w1);
       }
 #pragma unroll
       for (int u = 0; u < LB_TR / 32; ++u) {
         const i64 i = i0 + lane + 32 * u;
         if (i < j || i >= m) continue;
         R* p = at(i, j);
-        Cx<R> a = cld<R, CX>(p);
+        Sc<R> a = sc_ld<R, CX>(p);
         if (q.kind == 1) {
-          const Cx<R> li = cld<R, CX>(at(i, q.p));
+          const Sc<R> li = sc_ld<R, CX>(at(i, q.p));
           if (!FULL) {
             a = cfms_conj<R, CX>(a, li, w0);
             if (i == j) a.im = R(0);
           } else if (i > j) {
-            const Cx<R> lsi = cscale(li, q.dinv);
+            const Sc<R> lsi = cscale(li, q.dinv);
             a = csub(a, cscale(cmul<R, CX>(lsi, cconj(w0)), q.dg));
           } else {
-            a = Cx<R>{a.re - q.dg * cabs2(w0), R(0)};
+            a = Sc<R>{a.re - q.dg * cabs2(w0), R(0)};
           }
-          cst<R, CX>(p, a);
+          sc_st<R, CX>(p, a);
         } else if (q.kind == 2) {
-          const Cx<R> l0 = cld<R, CX>(at(i, q.p)), l1 = cld<R, CX>(at(i, q.p + 1));
+          const Sc<R> l0 = sc_ld<R, CX>(at(i, q.p)), l1 = sc_ld<R, CX>(at(i, q.p + 1));
           if (!FULL) {
             a = cfms_conj<R, CX>(cfms_conj<R, CX>(a, l0, w0), l1, w1);
           } else {
             a = csub(csub(a, cmul<R, CX>(l0, cconj(w0))), cmul<R, CX>(l1, cconj(w1)));
           }
           if (i == j) a.im = R(0);
-          cst<R, CX>(p, a);
+          sc_st<R, CX>(p, a);
         }
         if (i == j) {
           const R sc = FULL ? cabs2(a) : cabs1(a);
-          if ((FULL || diagonal) && fpl_better(sc, (long long)i, va, ia)) {
+          if ((FULL || diagonal) && better(sc, (long long)i, va, ia)) {
             va = sc;
             ia = i;
           }
         } else if (FULL) {
           const R sc = cabs2(a);
           const long long ix = i + j * (long long)m;
-          if (fpl_better(sc, ix, vb, ib)) {
+          if (better(sc, ix, vb, ib)) {
             vb = sc;
             ib = ix;
           }
         } else if (!diagonal && j == c) {
           const R sc = cabs1(a);
-          if (fpl_better(sc, (long long)i, vb, ib)) {
+          if (better(sc, (long long)i, vb, ib)) {
             vb = sc;
             ib = i;
           }
@@ -588,7 +530,7 @@ __global__ void __launch_bounds__(LB_THREADS, 1) lblt_rl_kernel(R* __restrict__ 
     long long bi = LLONG_MAX;
     for (i64 t = c + gt; t < m; t += T) {
       if (t == x) continue;
-      const R v = cabs1(t < x ? cld<R, CX>(at(x, t)) : cld<R, CX>(at(t, x)));
+      const R v = cabs1(t < x ? sc_ld<R, CX>(at(x, t)) : sc_ld<R, CX>(at(t, x)));
       if (v > bv) {
         bv = v;
         bi = t;
@@ -609,13 +551,13 @@ __global__ void __launch_bounds__(LB_THREADS, 1) lblt_rl_kernel(R* __restrict__ 
   // the new pending block after the interchanges; subdiag as the reference writes it
   auto take = [&](int c, int npiv) {
     if (npiv == 1) {
-      if (leader) cst<R, CX>(sd(c), Cx<R>{R(0), R(0)});
+      if (leader) sc_st<R, CX>(sd(c), Sc<R>{R(0), R(0)});
       return lb_one<R, CX>(c, __ldcg(at(c, c)));
     }
-    const Cx<R> a10 = cld<R, CX>(at(c + 1, c));
+    const Sc<R> a10 = sc_ld<R, CX>(at(c + 1, c));
     if (leader) {
-      cst<R, CX>(sd(c), a10);
-      cst<R, CX>(sd(c + 1), Cx<R>{R(0), R(0)});
+      sc_st<R, CX>(sd(c), a10);
+      sc_st<R, CX>(sd(c + 1), Sc<R>{R(0), R(0)});
     }
     return lb_two<R, CX>(c, __ldcg(at(c, c)), __ldcg(at(c + 1, c + 1)), a10);
   };
@@ -627,7 +569,7 @@ __global__ void __launch_bounds__(LB_THREADS, 1) lblt_rl_kernel(R* __restrict__ 
     // norm_max, then the whole matrix scaled by its recip, the first searches fused with the scaling
     R mx = R(0);
     for (i64 e = gt; e < (i64)m * m; e += T) {
-      const Cx<R> a = cld<R, CX>(at(e % m, e / m));
+      const Sc<R> a = sc_ld<R, CX>(at(e % m, e / m));
       const R v = fmax(fabs(a.re), fabs(a.im));  // norm_max: the largest |re| or |im| (faer-traits simd_abs_max)
       if (v > mx) mx = v;
     }
@@ -641,15 +583,15 @@ __global__ void __launch_bounds__(LB_THREADS, 1) lblt_rl_kernel(R* __restrict__ 
     long long ia = LLONG_MAX, ib = LLONG_MAX;
     for (i64 e = gt; e < (i64)m * m; e += T) {
       const i64 i = e % m, j = e / m;
-      const Cx<R> a = cscale(cld<R, CX>(at(i, j)), scale_bwd);
-      cst<R, CX>(at(i, j), a);
+      const Sc<R> a = cscale(sc_ld<R, CX>(at(i, j)), scale_bwd);
+      sc_st<R, CX>(at(i, j), a);
       const R sc = cabs2(a);
       if (i == j) {
-        if (fpl_better(sc, (long long)i, va, ia)) {
+        if (better(sc, (long long)i, va, ia)) {
           va = sc;
           ia = i;
         }
-      } else if (i > j && fpl_better(sc, (long long)e, vb, ib)) {
+      } else if (i > j && better(sc, (long long)e, vb, ib)) {
         vb = sc;
         ib = e;
       }
@@ -672,17 +614,17 @@ __global__ void __launch_bounds__(LB_THREADS, 1) lblt_rl_kernel(R* __restrict__ 
         const int sdx = (int)is;
         if (sdx != c) {
           for (i64 col = gt; col < c; col += T) {
-            const Cx<R> x = cld<R, CX>(at(c, col)), y = cld<R, CX>(at(sdx, col));
-            cst<R, CX>(at(c, col), y);
-            cst<R, CX>(at(sdx, col), x);
+            const Sc<R> x = sc_ld<R, CX>(at(c, col)), y = sc_ld<R, CX>(at(sdx, col));
+            sc_st<R, CX>(at(c, col), y);
+            sc_st<R, CX>(at(sdx, col), x);
           }
           if (leader) {
-            const Cx<R> x = cld<R, CX>(at(c, c)), y = cld<R, CX>(at(sdx, sdx));
-            cst<R, CX>(at(c, c), y);
-            cst<R, CX>(at(sdx, sdx), x);
+            const Sc<R> x = sc_ld<R, CX>(at(c, c)), y = sc_ld<R, CX>(at(sdx, sdx));
+            sc_st<R, CX>(at(c, c), y);
+            sc_st<R, CX>(at(sdx, sdx), x);
           }
         }
-        if (leader) cst<R, CX>(sd(c), Cx<R>{R(0), R(0)});
+        if (leader) sc_st<R, CX>(sd(c), Sc<R>{R(0), R(0)});
         record(c, sdx, -1, 1);
         c += 1;
         barrier();
@@ -690,7 +632,7 @@ __global__ void __launch_bounds__(LB_THREADS, 1) lblt_rl_kernel(R* __restrict__ 
           R bv = R(0);
           long long bi = LLONG_MAX;
           for (i64 t = c + gt; t < m; t += T) {
-            const R v = cabs2(cld<R, CX>(at(t, t)));
+            const R v = cabs2(sc_ld<R, CX>(at(t, t)));
             if (v > bv) {
               bv = v;
               bi = t;
@@ -761,7 +703,7 @@ __global__ void __launch_bounds__(LB_THREADS, 1) lblt_rl_kernel(R* __restrict__ 
             long long sx;
             lb_collect(set, gr, sx, s_v, s_i);
             if (sx == LLONG_MAX) sx = c;
-            if (cabs1(cld<R, CX>(at(i1, i1))) >= alpha * gr) {
+            if (cabs1(sc_ld<R, CX>(at(i1, i1))) >= alpha * gr) {
               npiv = 1;
               i0 = i1;
               i1 = -1;
@@ -815,8 +757,8 @@ __global__ void __launch_bounds__(LB_THREADS, 1) lblt_rl_kernel(R* __restrict__ 
   if (FULL) {
     barrier();
     for (i64 t = gt; t < m; t += T) {
-      cst<R, CX>(at(t, t), cscale(cld<R, CX>(at(t, t)), scale_fwd));
-      cst<R, CX>(sd(t), cscale(cld<R, CX>(sd(t)), scale_fwd));
+      sc_st<R, CX>(at(t, t), cscale(sc_ld<R, CX>(at(t, t)), scale_fwd));
+      sc_st<R, CX>(sd(t), cscale(sc_ld<R, CX>(sd(t)), scale_fwd));
     }
   }
 }
@@ -865,22 +807,22 @@ __global__ void lblt_block_solve_kernel(R* __restrict__ X, i64 n, i64 k, const R
     return;
   }
   R* x1 = X + W * (i + 1 + j * n);
-  Cx<R> s{sdg[W * i], CX ? sdg[W * i + 1] : R(0)};
+  Sc<R> s{sdg[W * i], CX ? sdg[W * i + 1] : R(0)};
   if (conj) s = cconj(s);
-  Cx<R> rk;  // recip(s)
+  Sc<R> rk;  // recip(s)
   if (!CX) {
-    rk = Cx<R>{R(1) / s.re, R(0)};
+    rk = Sc<R>{R(1) / s.re, R(0)};
   } else {
     const R den = s.re * s.re + s.im * s.im;
-    rk = Cx<R>{s.re / den, -s.im / den};
+    rk = Sc<R>{s.re / den, -s.im / den};
   }
-  const Cx<R> ak = cscale(cconj(rk), dg[W * i]);
-  const Cx<R> akp1 = cscale(rk, dg[W * (i + 1)]);
+  const Sc<R> ak = cscale(cconj(rk), dg[W * i]);
+  const Sc<R> akp1 = cscale(rk, dg[W * (i + 1)]);
   const R denom = R(1) / (cmul<R, CX>(ak, akp1).re - R(1));
-  const Cx<R> xk = cmul<R, CX>(Cx<R>{x0[0], CX ? x0[1] : R(0)}, cconj(rk));
-  const Cx<R> xkp1 = cmul<R, CX>(Cx<R>{x1[0], CX ? x1[1] : R(0)}, rk);
-  const Cx<R> y0 = cscale(csub(cmul<R, CX>(akp1, xk), xkp1), denom);
-  const Cx<R> y1 = cscale(csub(cmul<R, CX>(ak, xkp1), xk), denom);
+  const Sc<R> xk = cmul<R, CX>(Sc<R>{x0[0], CX ? x0[1] : R(0)}, cconj(rk));
+  const Sc<R> xkp1 = cmul<R, CX>(Sc<R>{x1[0], CX ? x1[1] : R(0)}, rk);
+  const Sc<R> y0 = cscale(csub(cmul<R, CX>(akp1, xk), xkp1), denom);
+  const Sc<R> y1 = cscale(csub(cmul<R, CX>(ak, xkp1), xk), denom);
   x0[0] = y0.re;
   x1[0] = y1.re;
   if (CX) {
@@ -908,10 +850,10 @@ __global__ void lblt_lb_kernel(R* __restrict__ out, i64 ors, i64 ocs, const R* _
   }
   R* o1 = out + W * (i * ors + (j + 1) * ocs);
   const R akp1 = L[W * ((j + 1) * lrs + (j + 1) * lcs)];
-  const Cx<R> s{sdg[W * j], CX ? sdg[W * j + 1] : R(0)};
-  const Cx<R> xk{o0[0], CX ? o0[1] : R(0)}, xkp1{o1[0], CX ? o1[1] : R(0)};
-  const Cx<R> y0 = cscale(xk, ak), y0b = cmul<R, CX>(xkp1, s);
-  const Cx<R> y1 = cscale(xkp1, akp1), y1b = cmul<R, CX>(xk, cconj(s));
+  const Sc<R> s{sdg[W * j], CX ? sdg[W * j + 1] : R(0)};
+  const Sc<R> xk{o0[0], CX ? o0[1] : R(0)}, xkp1{o1[0], CX ? o1[1] : R(0)};
+  const Sc<R> y0 = cscale(xk, ak), y0b = cmul<R, CX>(xkp1, s);
+  const Sc<R> y1 = cscale(xkp1, akp1), y1b = cmul<R, CX>(xk, cconj(s));
   o0[0] = y0.re + y0b.re;
   o1[0] = y1.re + y1b.re;
   if (CX) {
@@ -919,47 +861,6 @@ __global__ void lblt_lb_kernel(R* __restrict__ out, i64 ors, i64 ocs, const R* _
     o1[1] = y1.im + y1b.im;
   }
 }
-
-inline unsigned lb_blocks(i64 elems) { return (unsigned)((elems + 255) / 256); }
-
-// ---- the building blocks by scalar kind ----
-// dst(strict lower) -= W Al^H
-inline void lb_update(cudaStream_t st, VD dst, VCD Wv, VCD Al, std::false_type) {
-  gemm_f64(st, dst, STRICT_LOWER, 1, Wv, RECT, Al.t(), RECT, -1.0);
-}
-inline void lb_update(cudaStream_t st, VF dst, VCF Wv, VCF Al, std::false_type) {
-  gemm_f32(st, dst, STRICT_LOWER, 1, Wv, RECT, Al.t(), RECT, -1.0f);
-}
-inline void lb_update(cudaStream_t st, VD dst, VCD Wv, VCD Al, std::true_type) {
-  gemm_c64(st, dst, STRICT_LOWER, 1, Wv, RECT, false, Al.t(), RECT, true, -1.0, 0.0);
-}
-inline void lb_update(cudaStream_t st, VF dst, VCF Wv, VCF Al, std::true_type) {
-  gemm_c32(st, dst, STRICT_LOWER, 1, Wv, RECT, false, Al.t(), RECT, true, -1.0f, 0.0f);
-}
-// tmp(lower) = L(unit lower) X^H
-inline void lb_lxh(cudaStream_t st, VD tmp, VCD L, VCD X, std::false_type) { gemm_f64(st, tmp, TRI_LOWER, 0, L, UNIT_LOWER, X.t(), RECT, 1.0); }
-inline void lb_lxh(cudaStream_t st, VF tmp, VCF L, VCF X, std::false_type) { gemm_f32(st, tmp, TRI_LOWER, 0, L, UNIT_LOWER, X.t(), RECT, 1.0f); }
-inline void lb_lxh(cudaStream_t st, VD tmp, VCD L, VCD X, std::true_type) {
-  gemm_c64(st, tmp, TRI_LOWER, 0, L, UNIT_LOWER, false, X.t(), RECT, true, 1.0, 0.0);
-}
-inline void lb_lxh(cudaStream_t st, VF tmp, VCF L, VCF X, std::true_type) {
-  gemm_c32(st, tmp, TRI_LOWER, 0, L, UNIT_LOWER, false, X.t(), RECT, true, 1.0f, 0.0f);
-}
-inline void lb_lower(cudaStream_t st, VCD t, bool, VD rhs, std::false_type) { solve_lower_triangular_in_place_f64(st, t, true, rhs); }
-inline void lb_lower(cudaStream_t st, VCF t, bool, VF rhs, std::false_type) { solve_lower_triangular_in_place_f32(st, t, true, rhs); }
-inline void lb_lower(cudaStream_t st, VCD t, bool conj, VD rhs, std::true_type) { solve_lower_triangular_in_place_c64(st, t, true, conj, rhs); }
-inline void lb_lower(cudaStream_t st, VCF t, bool conj, VF rhs, std::true_type) { solve_lower_triangular_in_place_c32(st, t, true, conj, rhs); }
-inline void lb_upper(cudaStream_t st, VCD t, bool, VD rhs, std::false_type) { solve_upper_triangular_in_place_f64(st, t, true, rhs); }
-inline void lb_upper(cudaStream_t st, VCF t, bool, VF rhs, std::false_type) { solve_upper_triangular_in_place_f32(st, t, true, rhs); }
-inline void lb_upper(cudaStream_t st, VCD t, bool conj, VD rhs, std::true_type) { solve_upper_triangular_in_place_c64(st, t, true, conj, rhs); }
-inline void lb_upper(cudaStream_t st, VCF t, bool conj, VF rhs, std::true_type) { solve_upper_triangular_in_place_c32(st, t, true, conj, rhs); }
-
-template <class R, bool CX>
-View<R> lb_sub(View<R> v, i64 i, i64 j, i64 m, i64 n) {
-  return View<R>{v.ptr + (CX ? 2 : 1) * (i * v.rs + j * v.cs), m, n, v.rs, v.cs};
-}
-template <class R>
-View<const R> lb_c(View<R> v) { return View<const R>{v.ptr, v.nrows, v.ncols, v.rs, v.cs}; }
 
 template <class K>
 int lb_grid(K kernel, cudaStream_t st) {
@@ -978,7 +879,6 @@ enum LbStrategy : int { LB_PARTIAL = 0, LB_PARTIAL_DIAG = 1, LB_ROOK = 2, LB_ROO
 // pivots (host, n entries): the pivot row of each column, TOP_BIT set for the columns of 2 x 2 blocks.
 template <class R, bool CX>
 void lblt_in_place_t(cudaStream_t st, View<R> A, View<R> sub, int strategy, i64 block_size, std::vector<unsigned long long>& pivots) {
-  typedef std::integral_constant<bool, CX> Tag;
   constexpr int Wd = CX ? 2 : 1;
   const i64 n = A.nrows;
   FB_ASSERT(A.ncols == n && sub.nrows == n, "LBLT shape mismatch");
@@ -1046,11 +946,12 @@ void lblt_in_place_t(cudaStream_t st, View<R> A, View<R> sub, int strategy, i64 
         FB_CUDA_CHECK(cudaStreamSynchronize(st));
         const i64 mm = m - ks;
         if (mm > 0) {
-          View<R> dst = lb_sub<R, CX>(A, k + ks, k + ks, mm, mm);
+          View<R> dst = sub_t<R, CX>(A, k + ks, k + ks, mm, mm);
           View<const R> Wv{Wb + Wd * (i64)ks, mm, ks, 1, m};
-          lb_update(st, dst, Wv, lb_c(lb_sub<R, CX>(A, k + ks, k, mm, ks)), Tag());
+          const View<const R> Al = cview(sub_t<R, CX>(A, k + ks, k, mm, ks));
+          gemm_t<R, CX>(st, dst, STRICT_LOWER, 1, Wv, RECT, false, Al.t(), RECT, true, R(-1));  // dst(strict lower) -= W Al^H
           if (CX) {
-            lblt_real_diag_kernel<R><<<lb_blocks(mm), 256, 0, st>>>(dst.ptr, dst.rs, dst.cs, mm);
+            lblt_real_diag_kernel<R><<<grid_1d(mm), 256, 0, st>>>(dst.ptr, dst.rs, dst.cs, mm);
             FB_CUDA_CHECK(cudaGetLastError());
             note_launch();
           }
@@ -1096,7 +997,6 @@ std::vector<int> lb_kinds(const std::vector<unsigned char>& sd, i64 n) {
 template <class R, bool CX>
 void lblt_solve_t(cudaStream_t st, View<const R> L, const std::vector<unsigned char>& dgv, const std::vector<unsigned char>& sdv,
                   const long long* pf, const long long* pb, bool conj, View<R> rhs) {
-  typedef std::integral_constant<bool, CX> Tag;
   constexpr int Wd = CX ? 2 : 1;
   const i64 n = L.nrows, k = rhs.ncols;
   if (n == 0 || k == 0) return;
@@ -1114,13 +1014,13 @@ void lblt_solve_t(cudaStream_t st, View<const R> L, const std::vector<unsigned c
   FB_CUDA_CHECK(cudaMemcpyAsync(d_sd, sdv.data(), vb, cudaMemcpyHostToDevice, st));
   FB_CUDA_CHECK(cudaMemcpyAsync(d_kind, kind.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
   View<R> X{tmp, n, k, 1, n};
-  piv_gather_rows_t<R, CX>(st, X, lb_c(rhs), d_p);
-  lb_lower(st, L, conj, X, Tag());
-  lblt_block_solve_kernel<R, CX><<<lb_blocks(n * k), 256, 0, st>>>(tmp, n, k, d_dg, d_sd, d_kind, conj ? 1 : 0);
+  piv_gather_rows_t<R, CX>(st, X, cview(rhs), d_p);
+  solve_lower_t<R, CX>(st, L, true, conj, X);
+  lblt_block_solve_kernel<R, CX><<<grid_1d(n * k), 256, 0, st>>>(tmp, n, k, d_dg, d_sd, d_kind, conj ? 1 : 0);
   FB_CUDA_CHECK(cudaGetLastError());
   note_launch();
-  lb_upper(st, L.t(), !conj, X, Tag());
-  piv_gather_rows_t<R, CX>(st, rhs, lb_c(X), d_p + n);
+  solve_upper_t<R, CX>(st, L.t(), true, !conj, X);
+  piv_gather_rows_t<R, CX>(st, rhs, cview(X), d_p + n);
   FB_CUDA_CHECK(cudaStreamSynchronize(st));
   ws_free(tmp);
   ws_free(aux);
@@ -1129,7 +1029,6 @@ void lblt_solve_t(cudaStream_t st, View<const R> L, const std::vector<unsigned c
 // out <- P^T (L B L^H) P in the lower triangle, L B in the strict upper triangle (reconstruct.rs:12-87). pb: host perm_bwd.
 template <class R, bool CX>
 void lblt_reconstruct_t(cudaStream_t st, View<R> out, View<const R> L, const std::vector<unsigned char>& sdv, const long long* pb) {
-  typedef std::integral_constant<bool, CX> Tag;
   constexpr int Wd = CX ? 2 : 1;
   const i64 n = L.nrows;
   if (n == 0) return;
@@ -1143,17 +1042,17 @@ void lblt_reconstruct_t(cudaStream_t st, View<R> out, View<const R> L, const std
   FB_CUDA_CHECK(cudaMemcpyAsync(d_p, pb, (size_t)n * 8, cudaMemcpyHostToDevice, st));
   FB_CUDA_CHECK(cudaMemcpyAsync(d_sd, sdv.data(), vb, cudaMemcpyHostToDevice, st));
   FB_CUDA_CHECK(cudaMemcpyAsync(d_kind, kind.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
-  lblt_init_kernel<R, CX><<<lb_blocks(n * n), 256, 0, st>>>(out.ptr, out.rs, out.cs, L.ptr, L.rs, L.cs, n);
+  lblt_init_kernel<R, CX><<<grid_1d(n * n), 256, 0, st>>>(out.ptr, out.rs, out.cs, L.ptr, L.rs, L.cs, n);
   FB_CUDA_CHECK(cudaGetLastError());
   note_launch();
-  lblt_lb_kernel<R, CX><<<lb_blocks(n * n), 256, 0, st>>>(out.ptr, out.rs, out.cs, L.ptr, L.rs, L.cs, n, d_sd, d_kind);
+  lblt_lb_kernel<R, CX><<<grid_1d(n * n), 256, 0, st>>>(out.ptr, out.rs, out.cs, L.ptr, L.rs, L.cs, n, d_sd, d_kind);
   FB_CUDA_CHECK(cudaGetLastError());
   note_launch();
   View<R> Tm{tmp, n, n, 1, n};
-  lb_lxh(st, Tm, L, lb_c(out), Tag());
+  gemm_t<R, CX>(st, Tm, TRI_LOWER, 0, L, UNIT_LOWER, false, cview(out).t(), RECT, true, R(1));  // tmp(lower) = L(unit lower) X^H
   piv_sym_gather_t<R, CX>(st, out, tmp, n, d_p);
   if (CX) {
-    lblt_real_diag_kernel<R><<<lb_blocks(n), 256, 0, st>>>(out.ptr, out.rs, out.cs, n);
+    lblt_real_diag_kernel<R><<<grid_1d(n), 256, 0, st>>>(out.ptr, out.rs, out.cs, n);
     FB_CUDA_CHECK(cudaGetLastError());
     note_launch();
   }
@@ -1168,7 +1067,7 @@ void lblt_inverse_t(cudaStream_t st, View<R> out, View<const R> L, const std::ve
                     const std::vector<unsigned char>& sdv, const long long* pf, const long long* pb) {
   const i64 n = L.nrows;
   if (n == 0) return;
-  lblt_init_kernel<R, CX><<<lb_blocks(n * n), 256, 0, st>>>(out.ptr, out.rs, out.cs, nullptr, 0, 0, n);
+  lblt_init_kernel<R, CX><<<grid_1d(n * n), 256, 0, st>>>(out.ptr, out.rs, out.cs, nullptr, 0, 0, n);
   FB_CUDA_CHECK(cudaGetLastError());
   note_launch();
   lblt_solve_t<R, CX>(st, L, dgv, sdv, pf, pb, false, out);
@@ -1194,13 +1093,6 @@ std::vector<unsigned char> lb_read_vec(const void* p, size_t n, ptrdiff_t stride
   return out;
 }
 
-std::vector<long long> lb_read_perm(FaerV0_24_SliceRef s, size_t n, int idx_bytes) {
-  FB_ASSERT(n == 0 || s.ptr != nullptr, "null permutation slice");
-  std::vector<long long> p = read_perm(s.ptr, n, idx_bytes);
-  for (size_t i = 0; i < n; ++i) FB_ASSERT(p[i] >= 0 && (size_t)p[i] < n, "invalid permutation entry");
-  return p;
-}
-
 template <class R, bool CX>
 FaerV0_24_LbltStatus lblt_factor_entry(FaerV0_24_MatMut A, FaerV0_24_VecMut subdiag, FaerV0_24_SliceMut perm_fwd,
                                        FaerV0_24_SliceMut perm_bwd, FaerV0_24_LbltParams params, int idx_bytes) {
@@ -1223,17 +1115,15 @@ FaerV0_24_LbltStatus lblt_factor_entry(FaerV0_24_MatMut A, FaerV0_24_VecMut subd
   lblt_in_place_t<R, CX>(st, a.view<R>(), s.view<R>(), (int)params.pivoting, (i64)params.block_size, piv);
   finish_all(st, {&a, &s});
   // perm_fwd / perm_bwd / transposition_count from the pivots (factor.rs:1214-1227)
-  std::vector<long long> perm(n), inv(n);
-  for (size_t i = 0; i < n; ++i) perm[i] = (long long)i;
+  std::vector<long long> trans(n), fwd, bwd;
   size_t count = 0;
   for (size_t i = 0; i < n; ++i) {
-    const size_t p = (size_t)(piv[i] & ~(1ull << 63));
-    if (p != i) ++count;
-    std::swap(perm[i], perm[p]);
+    trans[i] = (long long)(piv[i] & ~(1ull << 63));
+    count += (size_t)trans[i] != i;
   }
-  for (size_t i = 0; i < n; ++i) inv[(size_t)perm[i]] = (long long)i;
-  write_perm(perm_fwd.ptr, perm, idx_bytes);
-  write_perm(perm_bwd.ptr, inv, idx_bytes);
+  perm_from_transpositions(n, trans, fwd, bwd);
+  write_perm(perm_fwd.ptr, fwd, idx_bytes);
+  write_perm(perm_bwd.ptr, bwd, idx_bytes);
   out.ok.transposition_count = count;
   return out;
 }
@@ -1248,7 +1138,7 @@ void lblt_solve_entry(FaerV0_24_MatRef L, FaerV0_24_VecRef diag, FaerV0_24_VecRe
   if (n == 0 || rhs.ncols == 0) return;
   cudaStream_t st = current_stream();
   const size_t es = (CX ? 2 : 1) * sizeof(R);
-  const std::vector<long long> pf = lb_read_perm(perm_fwd, n, idx_bytes), pb = lb_read_perm(perm_bwd, n, idx_bytes);
+  const std::vector<long long> pf = read_perm_checked(perm_fwd, n, idx_bytes), pb = read_perm_checked(perm_bwd, n, idx_bytes);
   const std::vector<unsigned char> dg = lb_read_vec(diag.ptr, n, diag.stride, es), sd = lb_read_vec(subdiag.ptr, n, subdiag.stride, es);
   StagedMat l(L.ptr, (i64)n, (i64)n, (i64)L.row_stride, (i64)L.col_stride, es, true, false, st);
   StagedMat r(rhs.ptr, (i64)rhs.nrows, (i64)rhs.ncols, (i64)rhs.row_stride, (i64)rhs.col_stride, es, true, true, st);
@@ -1267,7 +1157,7 @@ void lblt_recon_entry(FaerV0_24_MatMut A, FaerV0_24_MatRef L, FaerV0_24_VecRef d
   if (n == 0) return;
   cudaStream_t st = current_stream();
   const size_t es = (CX ? 2 : 1) * sizeof(R);
-  const std::vector<long long> pf = lb_read_perm(perm_fwd, n, idx_bytes), pb = lb_read_perm(perm_bwd, n, idx_bytes);
+  const std::vector<long long> pf = read_perm_checked(perm_fwd, n, idx_bytes), pb = read_perm_checked(perm_bwd, n, idx_bytes);
   const std::vector<unsigned char> sd = lb_read_vec(subdiag.ptr, n, subdiag.stride, es);
   // every entry of the output is written
   StagedMat a(A.ptr, (i64)n, (i64)n, (i64)A.row_stride, (i64)A.col_stride, es, false, true, st);
@@ -1279,13 +1169,6 @@ void lblt_recon_entry(FaerV0_24_MatMut A, FaerV0_24_MatRef L, FaerV0_24_VecRef d
     lblt_reconstruct_t<R, CX>(st, a.view<R>(), l.view<const R>(), sd, pb.data());
   }
   finish_all(st, {&a, &l});
-}
-
-// StackReq::and: the second request placed after the first at its alignment (as colpiv_qr.cu's cpq_and)
-inline FaerV0_24_Layout lb_and(FaerV0_24_Layout a, size_t b_bytes) {
-  const size_t al = a.align_bytes > 64 ? a.align_bytes : 64;
-  const size_t off = (a.len_bytes + 63) / 64 * 64;
-  return FaerV0_24_Layout{off + b_bytes, al};
 }
 
 }  // namespace
@@ -1300,7 +1183,7 @@ extern "C" {
     size_t bs = params.block_size;                                                                                                    \
     if (bs < 2 || dim <= bs) bs = 0;                                                                                                  \
     /* StackReq::new::<usize>(dim).and(temp_mat_scratch::<T>(dim, bs)) */                                                             \
-    return lb_and(FaerV0_24_Layout{dim * sizeof(size_t), alignof(size_t)}, dim * bs * (CX ? 2 : 1) * sizeof(R));                      \
+    return layout_and(FaerV0_24_Layout{dim * sizeof(size_t), alignof(size_t)}, dim * bs * (CX ? 2 : 1) * sizeof(R));                  \
   }                                                                                                                                   \
   FaerV0_24_LbltStatus libfaer_v0_23_lblt_factor_in_place_##IT##_##SUF(FaerV0_24_MatMut A, FaerV0_24_VecMut subdiag,                   \
                                                                        FaerV0_24_SliceMut perm_fwd, FaerV0_24_SliceMut perm_bwd,     \

@@ -13,45 +13,12 @@
 // on the host in tests/test_ldlt_types_emul_cpu.py): functional, not tuned — three launches per column, the trailing update one
 // thread per element instead of a GEMM. Solve / reconstruct / inverse are compositions of the structured products and triangular
 // solves of each scalar kind with the small bodies of ldlt_core.cuh in between.
-#include <type_traits>
-
 #include "flat_map.cuh"
 #include "ldlt_core.cuh"
 #include "runtime.cuh"
 #include "tensor_ops.cuh"
 
 namespace fb {
-
-namespace {
-
-typedef std::false_type Real;
-typedef std::true_type Cplx;
-
-// alpha = 1, Replace
-inline void lt_gemm(cudaStream_t st, VD dst, int ds, VCD a, int as, bool ca, VCD b, int bs, bool cb, Real) {
-  (void)ca; (void)cb;
-  gemm_f64(st, dst, ds, 0, a, as, b, bs, 1.0);
-}
-inline void lt_gemm(cudaStream_t st, VF dst, int ds, VCF a, int as, bool ca, VCF b, int bs, bool cb, Real) {
-  (void)ca; (void)cb;
-  gemm_f32(st, dst, ds, 0, a, as, b, bs, 1.0f);
-}
-inline void lt_gemm(cudaStream_t st, VD dst, int ds, VCD a, int as, bool ca, VCD b, int bs, bool cb, Cplx) {
-  gemm_c64(st, dst, ds, 0, a, as, ca, b, bs, cb, 1.0, 0.0);
-}
-inline void lt_gemm(cudaStream_t st, VF dst, int ds, VCF a, int as, bool ca, VCF b, int bs, bool cb, Cplx) {
-  gemm_c32(st, dst, ds, 0, a, as, ca, b, bs, cb, 1.0f, 0.0f);
-}
-inline void lt_solve_lower(cudaStream_t st, VCD t, bool unit, bool conj, VD rhs, Real) { (void)conj; solve_lower_triangular_in_place_f64(st, t, unit, rhs); }
-inline void lt_solve_lower(cudaStream_t st, VCF t, bool unit, bool conj, VF rhs, Real) { (void)conj; solve_lower_triangular_in_place_f32(st, t, unit, rhs); }
-inline void lt_solve_lower(cudaStream_t st, VCD t, bool unit, bool conj, VD rhs, Cplx) { solve_lower_triangular_in_place_c64(st, t, unit, conj, rhs); }
-inline void lt_solve_lower(cudaStream_t st, VCF t, bool unit, bool conj, VF rhs, Cplx) { solve_lower_triangular_in_place_c32(st, t, unit, conj, rhs); }
-inline void lt_solve_upper(cudaStream_t st, VCD t, bool unit, bool conj, VD rhs, Real) { (void)conj; solve_upper_triangular_in_place_f64(st, t, unit, rhs); }
-inline void lt_solve_upper(cudaStream_t st, VCF t, bool unit, bool conj, VF rhs, Real) { (void)conj; solve_upper_triangular_in_place_f32(st, t, unit, rhs); }
-inline void lt_solve_upper(cudaStream_t st, VCD t, bool unit, bool conj, VD rhs, Cplx) { solve_upper_triangular_in_place_c64(st, t, unit, conj, rhs); }
-inline void lt_solve_upper(cudaStream_t st, VCF t, bool unit, bool conj, VF rhs, Cplx) { solve_upper_triangular_in_place_c32(st, t, unit, conj, rhs); }
-
-}  // namespace
 
 // In-place LDLT of the lower triangle of A (device view, strides in elements). d_signs: device int8[n] or null.
 template <class R, bool CX>
@@ -89,23 +56,21 @@ LdltResult ldlt_in_place_t(cudaStream_t st, View<R> A, R delta, R eps, const sig
 // rhs <- conj?(A)^-1 rhs from the factors; D: device pointer to T-typed entries `dstride` elements apart (the real parts are used)
 template <class R, bool CX>
 void ldlt_solve_in_place_t(cudaStream_t st, View<const R> L, const R* D, i64 dstride, bool conj, View<R> rhs) {
-  typedef std::integral_constant<bool, CX> Tag;
   const i64 n = L.nrows, k = rhs.ncols;
   FB_ASSERT(L.ncols == n && rhs.nrows == n, "LDLT solve shape mismatch");
   if (n == 0 || k == 0) return;
   DevRun run{st};
   R* dinv = (R*)ws_alloc((size_t)n * sizeof(R));
   run(ldl::RecipDiag<R, CX>{D, dstride, n, dinv}, n, 1);
-  lt_solve_lower(st, L, true, conj, rhs, Tag());
+  solve_lower_t<R, CX>(st, L, true, conj, rhs);
   run(ldl::ScaleRows<R, CX>{rhs.ptr, rhs.rs, rhs.cs, n, k, dinv}, n, k);
-  lt_solve_upper(st, L.t(), true, !conj, rhs, Tag());
+  solve_upper_t<R, CX>(st, L.t(), true, !conj, rhs);
   FB_CUDA_CHECK(cudaStreamSynchronize(st));
   ws_free(dinv);
 }
 
 template <class R, bool CX>
 void ldlt_reconstruct_t(cudaStream_t st, View<R> out, View<const R> L, const R* D, i64 dstride) {
-  typedef std::integral_constant<bool, CX> Tag;
   const i64 n = out.nrows;
   FB_ASSERT(out.ncols == n && L.nrows == n && L.ncols == n, "ldlt_reconstruct shape mismatch");
   if (n == 0) return;
@@ -113,14 +78,13 @@ void ldlt_reconstruct_t(cudaStream_t st, View<R> out, View<const R> L, const R* 
   DevRun run{st};
   R* buf = (R*)ws_alloc((size_t)n * (size_t)n * W * sizeof(R));
   run(ldl::BuildLxD<R, CX>{L.ptr, L.rs, L.cs, D, dstride, buf, n, n}, n, n);
-  lt_gemm(st, out, TRI_LOWER, View<const R>{buf, n, n, 1, n}, TRI_LOWER, false, L.t(), UNIT_UPPER, true, Tag());  // (L D) * adjoint(L)
+  gemm_t<R, CX>(st, out, TRI_LOWER, 0, View<const R>{buf, n, n, 1, n}, TRI_LOWER, false, L.t(), UNIT_UPPER, true, R(1));  // (L D) * adjoint(L)
   FB_CUDA_CHECK(cudaStreamSynchronize(st));
   ws_free(buf);
 }
 
 template <class R, bool CX>
 void ldlt_inverse_t(cudaStream_t st, View<R> out, View<const R> L, const R* D, i64 dstride) {
-  typedef std::integral_constant<bool, CX> Tag;
   const i64 n = out.nrows;
   FB_ASSERT(out.ncols == n && L.nrows == n && L.ncols == n, "ldlt_inverse shape mismatch");
   if (n == 0) return;
@@ -130,11 +94,11 @@ void ldlt_inverse_t(cudaStream_t st, View<R> out, View<const R> L, const R* D, i
   R* dinv = (R*)ws_alloc((size_t)n * sizeof(R));
   View<R> M{buf, n, n, 1, n};
   run(ldl::SetIdentity<R, CX>{buf, n, n}, n, n);
-  lt_solve_lower(st, L, true, false, M, Tag());  // M = L^-1: unit lower, exact zeros above the diagonal
+  solve_lower_t<R, CX>(st, L, true, false, M);  // M = L^-1: unit lower, exact zeros above the diagonal
   run(ldl::RecipDiag<R, CX>{D, dstride, n, dinv}, n, 1);
   run(ldl::FillUpperAdjoint<R, CX>{buf, n, n, dinv}, n, n);
   const View<const R> Mc{buf, n, n, 1, n};
-  lt_gemm(st, out, TRI_LOWER, Mc, TRI_UPPER, false, Mc, UNIT_LOWER, false, Tag());  // (M^H D^-1) * M
+  gemm_t<R, CX>(st, out, TRI_LOWER, 0, Mc, TRI_UPPER, false, Mc, UNIT_LOWER, false, R(1));  // (M^H D^-1) * M
   FB_CUDA_CHECK(cudaStreamSynchronize(st));
   ws_free(dinv);
   ws_free(buf);

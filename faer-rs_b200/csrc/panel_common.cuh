@@ -17,11 +17,15 @@ template <> struct TLim<float> {
   __device__ static float min_pos() { return 1.17549435e-38f; }
   __device__ static float eps() { return 1.1920929e-7f; }
   __device__ static float inf() { return __int_as_float(0x7f800000); }
+  __device__ static float sqrt_min() { return 0x1p-63f; }  // sqrt_min_positive / sqrt_max_positive of faer's scaled norms
+  __device__ static float sqrt_max() { return 0x1p63f; }
 };
 template <> struct TLim<double> {
   __device__ static double min_pos() { return 2.2250738585072014e-308; }
   __device__ static double eps() { return 2.220446049250313e-16; }
   __device__ static double inf() { return __longlong_as_double(0x7ff0000000000000ll); }
+  __device__ static double sqrt_min() { return 0x1p-511; }
+  __device__ static double sqrt_max() { return 0x1p511; }
 };
 // loads of data written by OTHER CTAs of the same (persistent) kernel must bypass the non-coherent L1
 __device__ __forceinline__ float t_ldcg(const float* p) { return __ldcg(p); }

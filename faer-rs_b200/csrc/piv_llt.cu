@@ -31,6 +31,7 @@
 #include "panel_common.cuh"
 #include "piv_common.cuh"
 #include "runtime.cuh"
+#include "scalar.cuh"
 #include "tensor_ops.cuh"
 
 namespace fb {
@@ -42,13 +43,6 @@ constexpr int PIV_WARPS = PIV_THREADS / 32;
 // Widest panel the kernel takes: larger block sizes are clamped to it (the pivots depend on the block size only through the
 // rounding of the trailing updates).
 constexpr int PIV_MAX_BS = 256;
-
-__device__ __forceinline__ double add_rn(double a, double b) { return __dadd_rn(a, b); }
-__device__ __forceinline__ float add_rn(float a, float b) { return __fadd_rn(a, b); }
-__device__ __forceinline__ double sub_rn(double a, double b) { return __dsub_rn(a, b); }
-__device__ __forceinline__ float sub_rn(float a, float b) { return __fsub_rn(a, b); }
-__device__ __forceinline__ double mul_rn(double a, double b) { return __dmul_rn(a, b); }
-__device__ __forceinline__ float mul_rn(float a, float b) { return __fmul_rn(a, b); }
 
 // per-CTA argmax record, read by every CTA after the barrier
 template <class R>
@@ -383,20 +377,20 @@ __global__ void piv_sym_gather_kernel(R* __restrict__ out, i64 ors, i64 ocs, con
   if (CX) o[1] = direct ? q[1] : -q[1];
 }
 
-// ---- the building blocks by scalar kind ----
+// dst(i, j) = src(i, j) over an m x n block (strided views in units of the scalar kind)
 template <class R, bool CX>
-View<R> piv_sub(View<R> v, i64 i, i64 j, i64 m, i64 n) {
-  return View<R>{v.ptr + (CX ? 2 : 1) * (i * v.rs + j * v.cs), m, n, v.rs, v.cs};
+__global__ void piv_copy_kernel(R* __restrict__ dst, i64 drs, i64 dcs, const R* __restrict__ src, i64 srs, i64 scs, i64 m, i64 n) {
+  constexpr int W = CX ? 2 : 1;
+  const i64 e = (i64)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= m * n) return;
+  const i64 i = e % m, j = e / m;
+  const R* q = src + W * (i * srs + j * scs);
+  R* p = dst + W * (i * drs + j * dcs);
+  p[0] = q[0];
+  if (CX) p[1] = q[1];
 }
-// dst(lower) -= P P^H
-inline void piv_syrk(cudaStream_t st, VD dst, VCD P, std::false_type) { gemm_f64(st, dst, TRI_LOWER, 1, P, RECT, P.t(), RECT, -1.0); }
-inline void piv_syrk(cudaStream_t st, VF dst, VCF P, std::false_type) { gemm_f32(st, dst, TRI_LOWER, 1, P, RECT, P.t(), RECT, -1.0f); }
-inline void piv_syrk(cudaStream_t st, VD dst, VCD P, std::true_type) {
-  gemm_c64(st, dst, TRI_LOWER, 1, P, RECT, false, P.t(), RECT, true, -1.0, 0.0);
-}
-inline void piv_syrk(cudaStream_t st, VF dst, VCF P, std::true_type) {
-  gemm_c32(st, dst, TRI_LOWER, 1, P, RECT, false, P.t(), RECT, true, -1.0f, 0.0f);
-}
+
+// ---- the building blocks by scalar kind ----
 // L y = b, then L^H x = y, under A_conj (llt/solve.rs, the unpivoted solves)
 inline void piv_llt_solve(cudaStream_t st, VCD L, bool, VD rhs, std::false_type) { llt_solve_in_place_f64(st, L, rhs); }
 inline void piv_llt_solve(cudaStream_t st, VCF L, bool, VF rhs, std::false_type) { llt_solve_in_place_f32(st, L, rhs); }
@@ -414,15 +408,13 @@ void piv_llt_product<double, false>(cudaStream_t st, View<double> tmp, View<cons
   else llt_reconstruct_f64(st, tmp, L);
 }
 
-inline unsigned piv_blocks(i64 elems) { return (unsigned)((elems + 255) / 256); }
-
 }  // namespace
 
-// ---- piv_common.cuh: the one entry to the kernels above, for this file and lblt.cu ----
+// ---- piv_common.cuh: the one entry to the kernels above, for this file and the other pivoted factorizations ----
 template <class R, bool CX>
 void piv_laswp_t(cudaStream_t st, View<R> A, i64 k, i64 nt, const long long* hist) {
   if (k == 0 || nt == 0) return;
-  piv_llt_laswp_kernel<R, CX><<<piv_blocks(k), 256, 0, st>>>(A.ptr, A.rs, A.cs, (int)k, (int)nt, hist);
+  piv_llt_laswp_kernel<R, CX><<<grid_1d(k), 256, 0, st>>>(A.ptr, A.rs, A.cs, (int)k, (int)nt, hist);
   FB_CUDA_CHECK(cudaGetLastError());
   note_launch();
 }
@@ -430,7 +422,7 @@ template <class R, bool CX>
 void piv_gather_rows_t(cudaStream_t st, View<R> dst, View<const R> src, const long long* perm) {
   const i64 n = dst.nrows, k = dst.ncols;
   if (n == 0 || k == 0) return;
-  piv_gather_rows_kernel<R, CX><<<piv_blocks(n * k), 256, 0, st>>>(dst.ptr, dst.rs, dst.cs, src.ptr, src.rs, src.cs, n, k, perm);
+  piv_gather_rows_kernel<R, CX><<<grid_1d(n * k), 256, 0, st>>>(dst.ptr, dst.rs, dst.cs, src.ptr, src.rs, src.cs, n, k, perm);
   FB_CUDA_CHECK(cudaGetLastError());
   note_launch();
 }
@@ -438,14 +430,23 @@ template <class R, bool CX>
 void piv_sym_gather_t(cudaStream_t st, View<R> out, const R* tmp, i64 ld, const long long* p) {
   const i64 n = out.nrows;
   if (n == 0) return;
-  piv_sym_gather_kernel<R, CX><<<piv_blocks(n * n), 256, 0, st>>>(out.ptr, out.rs, out.cs, tmp, ld, n, p);
+  piv_sym_gather_kernel<R, CX><<<grid_1d(n * n), 256, 0, st>>>(out.ptr, out.rs, out.cs, tmp, ld, n, p);
+  FB_CUDA_CHECK(cudaGetLastError());
+  note_launch();
+}
+template <class R, bool CX>
+void piv_copy_t(cudaStream_t st, View<R> dst, View<const R> src) {
+  const i64 m = dst.nrows, n = dst.ncols;
+  if (m == 0 || n == 0) return;
+  piv_copy_kernel<R, CX><<<grid_1d(m * n), 256, 0, st>>>(dst.ptr, dst.rs, dst.cs, src.ptr, src.rs, src.cs, m, n);
   FB_CUDA_CHECK(cudaGetLastError());
   note_launch();
 }
 #define FB_PIV_COMMON_INST(R, CX)                                                                          \
   template void piv_laswp_t<R, CX>(cudaStream_t, View<R>, i64, i64, const long long*);                      \
   template void piv_gather_rows_t<R, CX>(cudaStream_t, View<R>, View<const R>, const long long*);           \
-  template void piv_sym_gather_t<R, CX>(cudaStream_t, View<R>, const R*, i64, const long long*);
+  template void piv_sym_gather_t<R, CX>(cudaStream_t, View<R>, const R*, i64, const long long*);            \
+  template void piv_copy_t<R, CX>(cudaStream_t, View<R>, View<const R>);
 FB_PIV_COMMON_INST(double, false)
 FB_PIV_COMMON_INST(float, false)
 FB_PIV_COMMON_INST(double, true)
@@ -459,16 +460,14 @@ struct PivLltResult {
 };
 
 // In-place pivoted Cholesky of the lower triangle of A (views in element units of the scalar kind; complex: COMPLEX units on an
-// R* base). perm (host, n entries) receives perm_fwd: the identity with the transpositions made, also on an error.
+// R* base). trans (host) receives the transpositions made: n entries, or none on a NonPositivePivot { index: 0 }.
 template <class R, bool CX>
-PivLltResult piv_llt_in_place_t(cudaStream_t st, View<R> A, i64 block_size, std::vector<long long>& perm) {
-  typedef std::integral_constant<bool, CX> Tag;
+PivLltResult piv_llt_in_place_t(cudaStream_t st, View<R> A, i64 block_size, std::vector<long long>& trans) {
   const i64 n = A.nrows;
   FB_ASSERT(A.ncols == n, "pivoted LLT needs a square matrix");
   FB_ASSERT(block_size > 0, "PivLltParams.block_size must be positive");
   FB_ASSERT(n < (i64)INT_MAX, "pivoted LLT: dimension too large");
-  perm.resize((size_t)n);
-  for (i64 i = 0; i < n; ++i) perm[(size_t)i] = i;
+  trans.clear();
   PivLltResult res{0, n, 0};
   if (n == 0) return res;
   const int bs = (int)std::min<i64>(block_size, PIV_MAX_BS);
@@ -516,17 +515,16 @@ PivLltResult piv_llt_in_place_t(cudaStream_t st, View<R> A, i64 block_size, std:
     piv_laswp_t<R, CX>(st, A, k, b, w.hist);
     if (k + b < n) {
       const i64 m = n - k - b;
-      View<R> P = piv_sub<R, CX>(A, k + b, k, m, b);
-      piv_syrk(st, piv_sub<R, CX>(A, k + b, k + b, m, m), View<const R>{P.ptr, P.nrows, P.ncols, P.rs, P.cs}, Tag());
+      const View<const R> P = cview(sub_t<R, CX>(A, k + b, k, m, b));  // A22(lower) -= P P^H
+      gemm_t<R, CX>(st, sub_t<R, CX>(A, k + b, k + b, m, m), TRI_LOWER, 1, P, RECT, false, P.t(), RECT, true, R(-1));
     }
   }
 
-  std::vector<long long> hist((size_t)n);
+  trans.resize((size_t)n);
   FB_CUDA_CHECK(cudaMemcpyAsync(h_status, w.status, sizeof(h_status), cudaMemcpyDeviceToHost, st));
-  FB_CUDA_CHECK(cudaMemcpyAsync(hist.data(), w.hist, (size_t)n * 8, cudaMemcpyDeviceToHost, st));
+  FB_CUDA_CHECK(cudaMemcpyAsync(trans.data(), w.hist, (size_t)n * 8, cudaMemcpyDeviceToHost, st));
   FB_CUDA_CHECK(cudaStreamSynchronize(st));
   ws_free(buf);
-  for (i64 j = 0; j < n; ++j) std::swap(perm[(size_t)j], perm[(size_t)hist[(size_t)j]]);
   res.transposition_count = h_status[2];
   if (h_status[0] == 1) {
     res.state = 1;
@@ -595,31 +593,23 @@ FaerV0_24_PivLltStatus piv_llt_factor_entry(FaerV0_24_MatMut A, FaerV0_24_SliceM
   cudaStream_t st = current_stream();
   const size_t es = (CX ? 2 : 1) * sizeof(R);
   StagedMat a(A.ptr, (i64)A.nrows, (i64)A.ncols, (i64)A.row_stride, (i64)A.col_stride, es, true, true, st);
-  std::vector<long long> perm;
-  const PivLltResult r = piv_llt_in_place_t<R, CX>(st, a.view<R>(), (i64)params.block_size, perm);
+  std::vector<long long> trans, fwd, bwd;
+  const PivLltResult r = piv_llt_in_place_t<R, CX>(st, a.view<R>(), (i64)params.block_size, trans);
   finish_all(st, {&a});
+  perm_from_transpositions(A.nrows, trans, fwd, bwd);
   FaerV0_24_PivLltStatus out;
   memset(&out, 0, sizeof(out));
-  write_perm(perm_fwd.ptr, perm, idx_bytes);
+  write_perm(perm_fwd.ptr, fwd, idx_bytes);
   if (r.state == 1) {
     out.tag = FaerV0_24_PivLltStatus_NonPositivePivot;
     out.non_positive_pivot.index = (size_t)r.index;
     return out;
   }
-  std::vector<long long> inv(perm.size());
-  for (size_t i = 0; i < perm.size(); ++i) inv[(size_t)perm[i]] = (long long)i;
-  write_perm(perm_bwd.ptr, inv, idx_bytes);
+  write_perm(perm_bwd.ptr, bwd, idx_bytes);
   out.tag = FaerV0_24_PivLltStatus_Ok;
   out.ok.rank = (size_t)r.index;
   out.ok.transposition_count = (size_t)r.transposition_count;
   return out;
-}
-
-std::vector<long long> piv_read_perm(FaerV0_24_SliceRef s, size_t n, int idx_bytes) {
-  FB_ASSERT(n == 0 || s.ptr != nullptr, "null permutation slice");
-  std::vector<long long> p = read_perm(s.ptr, n, idx_bytes);
-  for (size_t i = 0; i < n; ++i) FB_ASSERT(p[i] >= 0 && (size_t)p[i] < n, "invalid permutation entry");
-  return p;
 }
 
 template <class R, bool CX>
@@ -629,7 +619,7 @@ void piv_llt_solve_entry(FaerV0_24_MatRef L, FaerV0_24_SliceRef perm_fwd, FaerV0
   FB_ASSERT(L.nrows == L.ncols && rhs.nrows == L.nrows, "pivoted LLT solve shape mismatch");
   cudaStream_t st = current_stream();
   const size_t es = (CX ? 2 : 1) * sizeof(R), n = L.nrows;
-  std::vector<long long> pf = piv_read_perm(perm_fwd, n, idx_bytes), pb = piv_read_perm(perm_bwd, n, idx_bytes);
+  std::vector<long long> pf = read_perm_checked(perm_fwd, n, idx_bytes), pb = read_perm_checked(perm_bwd, n, idx_bytes);
   StagedMat l(L.ptr, (i64)L.nrows, (i64)L.ncols, (i64)L.row_stride, (i64)L.col_stride, es, true, false, st);
   StagedMat r(rhs.ptr, (i64)rhs.nrows, (i64)rhs.ncols, (i64)rhs.row_stride, (i64)rhs.col_stride, es, true, true, st);
   piv_llt_solve_t<R, CX>(st, l.view<const R>(), pf.data(), pb.data(), A_conj == FaerV0_24_Conj_Yes, r.view<R>());
@@ -642,7 +632,7 @@ void piv_llt_recon_entry(FaerV0_24_MatMut A, FaerV0_24_MatRef L, FaerV0_24_Slice
   FB_ASSERT(L.nrows == L.ncols && A.nrows == L.nrows && A.ncols == L.nrows, "pivoted LLT reconstruct / inverse shape mismatch");
   cudaStream_t st = current_stream();
   const size_t es = (CX ? 2 : 1) * sizeof(R), n = L.nrows;
-  std::vector<long long> pb = piv_read_perm(perm_bwd, n, idx_bytes);
+  std::vector<long long> pb = read_perm_checked(perm_bwd, n, idx_bytes);
   // only the lower triangle is written: the rest of A must survive the round trip
   StagedMat a(A.ptr, (i64)A.nrows, (i64)A.ncols, (i64)A.row_stride, (i64)A.col_stride, es, true, true, st);
   StagedMat l(L.ptr, (i64)L.nrows, (i64)L.ncols, (i64)L.row_stride, (i64)L.col_stride, es, true, false, st);

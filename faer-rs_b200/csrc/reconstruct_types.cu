@@ -12,7 +12,6 @@
 //   qr/no_pivoting/inverse.rs:11-43     A^-1 = R^-1 Q^H; here as the QR solve applied to the identity (Q^H first, then R^-1)
 // Tests: tests/test_gpu_zzzzzzzzz_2_reconstruct_types.py.
 #include <algorithm>
-#include <type_traits>
 
 #include "flat_map.cuh"
 #include "runtime.cuh"
@@ -109,10 +108,6 @@ struct Kind {
   typedef View<R> V;
   typedef View<const R> VC;
 
-  static V sub(V v, i64 i, i64 j, i64 m, i64 n) { return V{v.ptr + W * (i * v.rs + j * v.cs), m, n, v.rs, v.cs}; }
-  static VC sub(VC v, i64 i, i64 j, i64 m, i64 n) { return VC{v.ptr + W * (i * v.rs + j * v.cs), m, n, v.rs, v.cs}; }
-  static VC c(V v) { return VC{v.ptr, v.nrows, v.ncols, v.rs, v.cs}; }
-
   static void set_identity(cudaStream_t st, V A) {
     const i64 n = A.nrows;
     DevRun run{st};
@@ -134,59 +129,41 @@ struct Kind {
   }
 };
 
-// ---- the building blocks by scalar kind (alpha = 1, Replace) ----
-inline void rt_gemm(cudaStream_t st, VF dst, int ds, VCF a, int as, bool ca, VCF b, int bs, bool cb, std::false_type) {
-  (void)ca; (void)cb;  // real: conjugation is the identity
-  gemm_f32(st, dst, ds, 0, a, as, b, bs, 1.0f);
-}
-inline void rt_gemm(cudaStream_t st, VF dst, int ds, VCF a, int as, bool ca, VCF b, int bs, bool cb, std::true_type) {
-  gemm_c32(st, dst, ds, 0, a, as, ca, b, bs, cb, 1.0f, 0.0f);
-}
-inline void rt_gemm(cudaStream_t st, VD dst, int ds, VCD a, int as, bool ca, VCD b, int bs, bool cb, std::true_type) {
-  gemm_c64(st, dst, ds, 0, a, as, ca, b, bs, cb, 1.0, 0.0);
-}
-inline void rt_solve_lower(cudaStream_t st, VCF t, bool unit, VF rhs, std::false_type) { solve_lower_triangular_in_place_f32(st, t, unit, rhs); }
-inline void rt_solve_lower(cudaStream_t st, VCF t, bool unit, VF rhs, std::true_type) { solve_lower_triangular_in_place_c32(st, t, unit, false, rhs); }
-inline void rt_solve_lower(cudaStream_t st, VCD t, bool unit, VD rhs, std::true_type) { solve_lower_triangular_in_place_c64(st, t, unit, false, rhs); }
-inline void rt_solve_upper(cudaStream_t st, VCF t, bool unit, VF rhs, std::false_type) { solve_upper_triangular_in_place_f32(st, t, unit, rhs); }
-inline void rt_solve_upper(cudaStream_t st, VCF t, bool unit, VF rhs, std::true_type) { solve_upper_triangular_in_place_c32(st, t, unit, false, rhs); }
-inline void rt_solve_upper(cudaStream_t st, VCD t, bool unit, VD rhs, std::true_type) { solve_upper_triangular_in_place_c64(st, t, unit, false, rhs); }
 // rhs <- Q rhs (adjoint = false) or Q^H rhs (adjoint = true); Q^H is the transposed sequence with Conj::Yes composed in
 // (householder.rs:768-808 as qr/no_pivoting/solve.rs:60-67 calls it)
-inline void rt_hh_seq(cudaStream_t st, VCF b, VCF f, VF rhs, bool adjoint, std::false_type) {
-  if (adjoint) apply_block_householder_sequence_transpose_on_the_left<float>(st, b, f, rhs);
-  else apply_block_householder_sequence_on_the_left<float>(st, b, f, rhs);
-}
-inline void rt_hh_seq(cudaStream_t st, VCF b, VCF f, VF rhs, bool adjoint, std::true_type) {
-  apply_householder_sequence_left_c32(st, b, f, adjoint, rhs, adjoint);
-}
-inline void rt_hh_seq(cudaStream_t st, VCD b, VCD f, VD rhs, bool adjoint, std::true_type) {
-  apply_householder_sequence_left_c64(st, b, f, adjoint, rhs, adjoint);
+template <class R, bool CX>
+void rt_hh_seq(cudaStream_t st, View<const R> b, View<const R> f, View<R> rhs, bool adjoint) {
+  if constexpr (!CX) {
+    if (adjoint) apply_block_householder_sequence_transpose_on_the_left<R>(st, b, f, rhs);
+    else apply_block_householder_sequence_on_the_left<R>(st, b, f, rhs);
+  } else if constexpr (sizeof(R) == 8) {
+    apply_householder_sequence_left_c64(st, b, f, adjoint, rhs, adjoint);
+  } else {
+    apply_householder_sequence_left_c32(st, b, f, adjoint, rhs, adjoint);
+  }
 }
 
 }  // namespace
 
 template <class R, bool CX>
 void llt_reconstruct_t(cudaStream_t st, View<R> out, View<const R> L) {
-  typedef std::integral_constant<bool, CX> Tag;
   const i64 n = out.nrows;
   FB_ASSERT(out.ncols == n && L.nrows == n && L.ncols == n, "llt_reconstruct shape mismatch");
   if (n == 0) return;
-  rt_gemm(st, out, TRI_LOWER, L, TRI_LOWER, false, L.t(), TRI_UPPER, true, Tag());  // L * adjoint(L)
+  gemm_t<R, CX>(st, out, TRI_LOWER, 0, L, TRI_LOWER, false, L.t(), TRI_UPPER, true, R(1));  // L * adjoint(L)
 }
 
 template <class R, bool CX>
 void llt_inverse_t(cudaStream_t st, View<R> out, View<const R> L) {
   typedef Kind<R, CX> K;
-  typedef std::integral_constant<bool, CX> Tag;
   const i64 n = out.nrows;
   FB_ASSERT(out.ncols == n && L.nrows == n && L.ncols == n, "llt_inverse shape mismatch");
   if (n == 0) return;
   R* buf = (R*)ws_alloc((size_t)n * (size_t)n * K::W * sizeof(R));
   View<R> Li{buf, n, n, 1, n};
   K::set_identity(st, Li);
-  rt_solve_lower(st, L, false, Li, Tag());  // L_inv: lower triangular, exact zeros above the diagonal
-  rt_gemm(st, out, TRI_LOWER, K::c(Li).t(), TRI_UPPER, true, K::c(Li), TRI_LOWER, false, Tag());  // adjoint(L_inv) * L_inv
+  solve_lower_t<R, CX>(st, L, false, false, Li);  // L_inv: lower triangular, exact zeros above the diagonal
+  gemm_t<R, CX>(st, out, TRI_LOWER, 0, cview(Li).t(), TRI_UPPER, true, cview(Li), TRI_LOWER, false, R(1));  // adjoint(L_inv) * L_inv
   FB_CUDA_CHECK(cudaStreamSynchronize(st));
   ws_free(buf);
 }
@@ -195,18 +172,17 @@ void llt_inverse_t(cudaStream_t st, View<R> out, View<const R> L) {
 template <class R, bool CX>
 void lu_reconstruct_t(cudaStream_t st, View<R> out, View<const R> L, View<const R> U, const long long* perm_bwd) {
   typedef Kind<R, CX> K;
-  typedef std::integral_constant<bool, CX> Tag;
   const i64 m = L.nrows, n = U.ncols, size = std::min(m, n);
   FB_ASSERT(out.nrows == m && out.ncols == n && L.ncols >= size && U.nrows >= size, "lu_reconstruct shape mismatch");
   if (m == 0 || n == 0) return;
-  rt_gemm(st, K::sub(out, 0, 0, size, size), RECT, K::sub(L, 0, 0, size, size), UNIT_LOWER, false, K::sub(U, 0, 0, size, size),
-          TRI_UPPER, false, Tag());
+  const View<const R> Ls = sub_t<R, CX>(L, 0, 0, size, size), Us = sub_t<R, CX>(U, 0, 0, size, size);
+  gemm_t<R, CX>(st, sub_t<R, CX>(out, 0, 0, size, size), RECT, 0, Ls, UNIT_LOWER, false, Us, TRI_UPPER, false, R(1));
   if (m > n)
-    rt_gemm(st, K::sub(out, size, 0, m - size, size), RECT, K::sub(L, size, 0, m - size, size), RECT, false,
-            K::sub(U, 0, 0, size, size), TRI_UPPER, false, Tag());
+    gemm_t<R, CX>(st, sub_t<R, CX>(out, size, 0, m - size, size), RECT, 0, sub_t<R, CX>(L, size, 0, m - size, size), RECT, false, Us,
+                  TRI_UPPER, false, R(1));
   if (m < n)
-    rt_gemm(st, K::sub(out, 0, size, size, n - size), RECT, K::sub(L, 0, 0, size, size), UNIT_LOWER, false,
-            K::sub(U, 0, size, size, n - size), RECT, false, Tag());
+    gemm_t<R, CX>(st, sub_t<R, CX>(out, 0, size, size, n - size), RECT, 0, Ls, UNIT_LOWER, false, sub_t<R, CX>(U, 0, size, size, n - size),
+                  RECT, false, R(1));
   // (P A)[i, :] = A[perm_fwd[i], :]  =>  A[j, :] = (L U)[perm_bwd[j], :]
   K::permute_rows(st, out, perm_bwd);
 }
@@ -214,59 +190,53 @@ void lu_reconstruct_t(cudaStream_t st, View<R> out, View<const R> L, View<const 
 template <class R, bool CX>
 void lu_inverse_t(cudaStream_t st, View<R> out, View<const R> L, View<const R> U, const long long* perm_fwd) {
   typedef Kind<R, CX> K;
-  typedef std::integral_constant<bool, CX> Tag;
   const i64 n = out.nrows;
   FB_ASSERT(out.ncols == n && L.nrows == n && L.ncols == n && U.nrows == n && U.ncols == n, "lu_inverse shape mismatch");
   if (n == 0) return;
   // lu/partial_pivoting/solve.rs:21-54 on the identity: rows permuted, unit-lower solve, upper solve
   K::set_identity(st, out);
   K::permute_rows(st, out, perm_fwd);
-  rt_solve_lower(st, L, true, out, Tag());
-  rt_solve_upper(st, U, false, out, Tag());
+  solve_lower_t<R, CX>(st, L, true, false, out);
+  solve_upper_t<R, CX>(st, U, false, false, out);
 }
 
 template <class R, bool CX>
 void qr_reconstruct_t(cudaStream_t st, View<R> out, View<const R> Qb, View<const R> Qc, View<const R> Rm) {
   typedef Kind<R, CX> K;
-  typedef std::integral_constant<bool, CX> Tag;
   const i64 m = Qb.nrows, n = Rm.ncols, size = std::min(m, n);
   FB_ASSERT(out.nrows == m && out.ncols == n && Qb.ncols == size && Qc.nrows > 0 && Qc.ncols == size && Rm.nrows == size,
             "qr_reconstruct shape mismatch");
   if (m == 0 || n == 0) return;
   DevRun run{st};
   run(RtSetUpperTrapezoid<R, K::W>{out.ptr, out.rs, out.cs, m, n, Rm.ptr, Rm.rs, Rm.cs, size}, m, n);
-  if (size > 0) rt_hh_seq(st, Qb, Qc, out, false, Tag());
+  if (size > 0) rt_hh_seq<R, CX>(st, Qb, Qc, out, false);
 }
 
 template <class R, bool CX>
 void qr_inverse_t(cudaStream_t st, View<R> out, View<const R> Qb, View<const R> Qc, View<const R> Rm) {
   typedef Kind<R, CX> K;
-  typedef std::integral_constant<bool, CX> Tag;
   const i64 n = out.nrows;
   FB_ASSERT(out.ncols == n && Qb.nrows == n && Qb.ncols == n && Qc.nrows > 0 && Qc.ncols == n && Rm.nrows == n && Rm.ncols == n,
             "qr_inverse shape mismatch");
   if (n == 0) return;
   K::set_identity(st, out);
-  rt_hh_seq(st, Qb, Qc, out, true, Tag());     // Q^H
-  rt_solve_upper(st, Rm, false, out, Tag());  // R^-1 Q^H
+  rt_hh_seq<R, CX>(st, Qb, Qc, out, true);          // Q^H
+  solve_upper_t<R, CX>(st, Rm, false, false, out);  // R^-1 Q^H
 }
 
 // linalg::triangular_inverse::invert_[unit_]{lower,upper}_triangular (triangular_inverse.rs): dst(triangle) <- src(triangle)^-1;
 // only the triangle is written (the diagonal too unless `unit`). Here as the triangular solve applied to the identity.
-inline void rt_solve_lower(cudaStream_t st, VCD t, bool unit, VD rhs, std::false_type) { solve_lower_triangular_in_place_f64(st, t, unit, rhs); }
-inline void rt_solve_upper(cudaStream_t st, VCD t, bool unit, VD rhs, std::false_type) { solve_upper_triangular_in_place_f64(st, t, unit, rhs); }
 template <class R, bool CX>
 void inverse_triangular_t(cudaStream_t st, View<R> dst, View<const R> src, bool lower, bool unit) {
   typedef Kind<R, CX> K;
-  typedef std::integral_constant<bool, CX> Tag;
   const i64 n = dst.nrows;
   FB_ASSERT(dst.ncols == n && src.nrows == n && src.ncols == n, "inverse_triangular shape mismatch");
   if (n == 0) return;
   R* buf = (R*)ws_alloc((size_t)n * (size_t)n * K::W * sizeof(R));
   View<R> X{buf, n, n, 1, n};
   K::set_identity(st, X);
-  if (lower) rt_solve_lower(st, src, unit, X, Tag());
-  else rt_solve_upper(st, src, unit, X, Tag());
+  if (lower) solve_lower_t<R, CX>(st, src, unit, false, X);
+  else solve_upper_t<R, CX>(st, src, unit, false, X);
   DevRun run{st};
   run(RtCopyTriangle<R, K::W>{dst.ptr, dst.rs, dst.cs, buf, 1, n, n, lower ? 1 : 0, unit ? 1 : 0}, n, n);
   FB_CUDA_CHECK(cudaStreamSynchronize(st));

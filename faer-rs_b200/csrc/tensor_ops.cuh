@@ -1,5 +1,6 @@
-// Type-generic spellings (f32 / f64) of the tensor-core building blocks, so that the Householder / QR drivers are written
-// once. f64 -> DMMA GEMM (gemm_f64.cu), f32 -> 3xTF32 GEMM (gemm_f32.cu); triangular solves from trsm.cu.
+// Type-generic spellings (f32 / f64, and every scalar kind <R, complex?>) of the tensor-core building blocks, so that the drivers
+// are written once. f64 -> DMMA GEMM (gemm_f64.cu), f32 -> 3xTF32 GEMM (gemm_f32.cu), c64 / c32 on those (gemm_c64.cu,
+// gemm_c32.cu); triangular solves from trsm.cu and cplx.cu.
 #pragma once
 #include "gemm_f32.cuh"
 #include "linalg_f64.cuh"
@@ -19,6 +20,36 @@ inline void solve_upper(cudaStream_t st, VCF t, bool unit, VF rhs) { solve_upper
 
 template <class T>
 inline View<const T> cview(const View<T>& v) { return View<const T>{v.ptr, v.nrows, v.ncols, v.rs, v.cs}; }
+
+// The same building blocks over the scalar kind <R, complex?>: <double, false> f64, <float, false> f32, <double, true> c64,
+// <float, true> c32 (complex views in COMPLEX element units on an R* base). Real kinds ignore the conjugation flags; complex
+// products take a real alpha.
+template <class R, bool CX>
+inline void gemm_t(cudaStream_t st, View<R> dst, int ds, int accum, View<const R> lhs, int ls, bool conj_lhs, View<const R> rhs,
+                   int rs, bool conj_rhs, R alpha) {
+  if constexpr (!CX) gemm(st, dst, ds, accum, lhs, ls, rhs, rs, alpha);
+  else if constexpr (sizeof(R) == 8) gemm_c64(st, dst, ds, accum, lhs, ls, conj_lhs, rhs, rs, conj_rhs, alpha, 0.0);
+  else gemm_c32(st, dst, ds, accum, lhs, ls, conj_lhs, rhs, rs, conj_rhs, alpha, 0.0f);
+}
+template <class R, bool CX>
+inline void solve_lower_t(cudaStream_t st, View<const R> t, bool unit, bool conj, View<R> rhs) {
+  if constexpr (!CX) solve_lower(st, t, unit, rhs);
+  else if constexpr (sizeof(R) == 8) solve_lower_triangular_in_place_c64(st, t, unit, conj, rhs);
+  else solve_lower_triangular_in_place_c32(st, t, unit, conj, rhs);
+}
+template <class R, bool CX>
+inline void solve_upper_t(cudaStream_t st, View<const R> t, bool unit, bool conj, View<R> rhs) {
+  if constexpr (!CX) solve_upper(st, t, unit, rhs);
+  else if constexpr (sizeof(R) == 8) solve_upper_triangular_in_place_c64(st, t, unit, conj, rhs);
+  else solve_upper_triangular_in_place_c32(st, t, unit, conj, rhs);
+}
+// the m x n block at (i, j)
+template <class R, bool CX>
+inline View<R> sub_t(View<R> v, i64 i, i64 j, i64 m, i64 n) { return View<R>{v.ptr + (CX ? 2 : 1) * (i * v.rs + j * v.cs), m, n, v.rs, v.cs}; }
+template <class R, bool CX>
+inline View<const R> sub_t(View<const R> v, i64 i, i64 j, i64 m, i64 n) {
+  return View<const R>{v.ptr + (CX ? 2 : 1) * (i * v.rs + j * v.cs), m, n, v.rs, v.cs};
+}
 
 // ---- householder.cu ----
 // T(strict upper) <- V^H V for the N reflectors stored in V (m x N, implicit unit diagonal, R above it is ignored);
