@@ -598,6 +598,44 @@ def load() -> C.CDLL:
                 f = getattr(lib, f"{pre}{name}_{it}_{suf}")
                 f.argtypes = [MatMut, MatRef, MatRef, SliceMut, SliceMut, SliceMut, SliceMut, P, MemAlloc]
                 f.restype = None
+    # double-double kinds (include/faer_b200_fx128.h)
+    for suf in ("fx128", "cx128"):
+        sig = {
+            "matmul": ([MatMut, C.c_int, MatRef, MatRef, C.c_void_p, P], None),
+            "matmul_triangular": ([MatMut, C.c_int, C.c_int, MatRef, C.c_int, MatRef, C.c_int, C.c_void_p, P], None),
+            "LltParams": ([], LltParams),
+            "llt_factor_in_place_scratch": ([C.c_size_t, P, LltParams], Layout),
+            "llt_factor_in_place": ([MatMut, LltRegularization, P, MemAlloc, LltParams], LltStatus),
+            "llt_solve_in_place_scratch": ([C.c_size_t, C.c_size_t, P], Layout),
+            "llt_solve_in_place": ([MatRef, C.c_int, MatMut, P, MemAlloc], None),
+            "llt_reconstruct_scratch": ([C.c_size_t, P], Layout),
+            "llt_reconstruct": ([MatMut, MatRef, P, MemAlloc], None),
+            "llt_inverse_scratch": ([C.c_size_t, P], Layout),
+            "llt_inverse": ([MatMut, MatRef, P, MemAlloc], None),
+            "PartialPivLuParams": ([], PartialPivLuParams),
+        }
+        for name in ("solve_triangular_lower", "solve_triangular_upper", "solve_unit_triangular_lower",
+                     "solve_unit_triangular_upper"):
+            sig[f"{name}_in_place"] = ([MatRef, C.c_int, MatMut, P], None)
+        for name in ("inverse_triangular_lower", "inverse_triangular_upper", "inverse_unit_triangular_lower",
+                     "inverse_unit_triangular_upper"):
+            sig[f"{name}_in_place"] = ([MatMut, MatRef, P], None)
+        for it in ("u32", "u64"):
+            sig[f"partial_piv_lu_factor_in_place_scratch_{it}"] = ([C.c_size_t, C.c_size_t, P, PartialPivLuParams], Layout)
+            sig[f"partial_piv_lu_factor_in_place_{it}"] = ([MatMut, SliceMut, SliceMut, P, MemAlloc, PartialPivLuParams],
+                                                           PartialPivLuStatus)
+            for name in ("solve", "solve_transpose"):
+                sig[f"partial_piv_lu_{name}_in_place_scratch_{it}"] = ([C.c_size_t, C.c_size_t, P], Layout)
+                sig[f"partial_piv_lu_{name}_in_place_{it}"] = ([MatRef, MatRef, C.c_int, SliceMut, SliceMut, MatMut, P,
+                                                                MemAlloc], None)
+            sig[f"partial_piv_lu_reconstruct_scratch_{it}"] = ([C.c_size_t, C.c_size_t, P], Layout)
+            sig[f"partial_piv_lu_inverse_scratch_{it}"] = ([C.c_size_t, P], Layout)
+            for name in ("reconstruct", "inverse"):
+                sig[f"partial_piv_lu_{name}_{it}"] = ([MatMut, MatRef, MatRef, SliceMut, SliceMut, P, MemAlloc], None)
+        for name, (args, res) in sig.items():
+            f = getattr(lib, f"libfaer_v0_23_{name}_{suf}")
+            f.argtypes = args
+            f.restype = res
     lib.faer_b200_version.argtypes = []
     lib.faer_b200_version.restype = C.c_char_p
     _lib = lib
@@ -610,8 +648,37 @@ def _is_torch(x: Any) -> bool:
     return type(x).__module__.startswith("torch")
 
 
+# Double-double element types. On the host: numpy structured dtypes, {hi, lo} per fx128 and {re.hi, re.lo, im.hi, im.lo} per cx128.
+FX128 = np.dtype([("hi", "<f8"), ("lo", "<f8")])
+CX128 = np.dtype([("re_hi", "<f8"), ("re_lo", "<f8"), ("im_hi", "<f8"), ("im_lo", "<f8")])
+
+
+class DDTensor:
+    """A CUDA (or CPU) float64 tensor seen as a matrix of fx128 (trailing limb axis of 2: [..., (hi, lo)]) or cx128 (trailing
+    axes 2 x 2: [..., (re, im), (hi, lo)]) elements; the limb axes must be contiguous. _fields turns it into element strides."""
+
+    def __init__(self, t, complex: bool = False):
+        limbs = 4 if complex else 2
+        assert t.dtype.is_floating_point and t.element_size() == 8, "double-double tensors are float64"
+        assert t.dim() == (4 if complex else 3) and t.shape[2:] == ((2, 2) if complex else (2,)), "bad limb axes"
+        inner = (2, 1) if complex else (1,)
+        assert tuple(t.stride()[2:]) == inner, "the limb axes must be contiguous"
+        assert t.stride(0) % limbs == 0 and t.stride(1) % limbs == 0, "element strides must be whole elements"
+        self.t, self.complex = t, complex
+
+    @property
+    def shape(self):
+        return tuple(self.t.shape[:2])
+
+
 def _fields(x: Any, itemsize_expected: int | None = None):
-    """(ptr, nrows, ncols, row_stride, col_stride) of a 2-D numpy array or torch tensor (strides in elements)."""
+    """(ptr, nrows, ncols, row_stride, col_stride) of a 2-D numpy array, torch tensor or DDTensor (strides in elements)."""
+    if isinstance(x, DDTensor):
+        limbs = 4 if x.complex else 2
+        if itemsize_expected is not None:
+            assert 8 * limbs == itemsize_expected
+        t = x.t
+        return t.data_ptr(), t.shape[0], t.shape[1], t.stride(0) // limbs, t.stride(1) // limbs
     if _is_torch(x):
         assert x.dim() == 2, "expected a 2-D tensor"
         if itemsize_expected is not None:

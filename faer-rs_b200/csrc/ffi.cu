@@ -767,11 +767,6 @@ FaerV0_24_PartialPivLuParams libfaer_v0_23_PartialPivLuParams_f64(void) {
   return FaerV0_24_PartialPivLuParams{16, 64, 128 * 128};
 }
 
-static FaerV0_24_Layout lu_scratch(size_t nrows, size_t ncols, size_t idx_bytes) {
-  // reference: StackReq::new::<I>(min(nrows, ncols)) (factor.rs:224-233)
-  size_t size = nrows < ncols ? nrows : ncols;
-  return FaerV0_24_Layout{size * idx_bytes, idx_bytes};
-}
 FaerV0_24_Layout libfaer_v0_23_partial_piv_lu_factor_in_place_scratch_u32_f64(size_t nrows, size_t ncols, FaerV0_24_Par par,
                                                                               FaerV0_24_PartialPivLuParams params) {
   (void)par; (void)params;

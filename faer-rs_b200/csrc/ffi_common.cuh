@@ -82,6 +82,11 @@ static inline void perm_from_transpositions(size_t len, const std::vector<long l
   for (size_t i = 0; i < len; ++i) bwd[(size_t)fwd[i]] = (long long)i;
 }
 
+// partial-pivoting LU factor scratch: StackReq::new::<I>(min(nrows, ncols)) (lu/partial_pivoting/factor.rs:224-233)
+static inline FaerV0_24_Layout lu_scratch(size_t nrows, size_t ncols, size_t idx_bytes) {
+  size_t size = nrows < ncols ? nrows : ncols;
+  return FaerV0_24_Layout{size * idx_bytes, idx_bytes};
+}
 // StackReq::and: the second request placed after the first at its alignment (dyn-stack's rule for equal alignments)
 static inline FaerV0_24_Layout layout_and(FaerV0_24_Layout a, size_t b_bytes) {
   const size_t al = a.align_bytes > 64 ? a.align_bytes : 64;

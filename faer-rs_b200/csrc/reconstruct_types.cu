@@ -13,6 +13,9 @@
 // Tests: tests/test_gpu_zzzzzzzzz_2_reconstruct_types.py.
 #include <algorithm>
 
+#if defined(__CUDACC__)
+#include "dd.cuh"
+#endif
 #include "flat_map.cuh"
 #include "runtime.cuh"
 #include "tensor_ops.cuh"
@@ -246,6 +249,10 @@ template void inverse_triangular_t<double, false>(cudaStream_t, View<double>, Vi
 template void inverse_triangular_t<float, false>(cudaStream_t, View<float>, View<const float>, bool, bool);
 template void inverse_triangular_t<double, true>(cudaStream_t, View<double>, View<const double>, bool, bool);
 template void inverse_triangular_t<float, true>(cudaStream_t, View<float>, View<const float>, bool, bool);
+#if defined(__CUDACC__)  // the host builds of this file (tools/emul) provide building blocks for the four other kinds only
+template void inverse_triangular_t<dd, false>(cudaStream_t, View<dd>, View<const dd>, bool, bool);
+template void inverse_triangular_t<dd, true>(cudaStream_t, View<dd>, View<const dd>, bool, bool);
+#endif
 
 #define FB_RECON_INST(R, CX)                                                                                                     \
   template void llt_reconstruct_t<R, CX>(cudaStream_t, View<R>, View<const R>);                                                  \
@@ -258,6 +265,16 @@ FB_RECON_INST(float, false)
 FB_RECON_INST(double, true)
 FB_RECON_INST(float, true)
 #undef FB_RECON_INST
+#if defined(__CUDACC__)  // double-double: the LLT and LU compositions (there is no dd Householder QR)
+#define FB_RECON_INST_DD(CX)                                                                                                     \
+  template void llt_reconstruct_t<dd, CX>(cudaStream_t, View<dd>, View<const dd>);                                               \
+  template void llt_inverse_t<dd, CX>(cudaStream_t, View<dd>, View<const dd>);                                                   \
+  template void lu_reconstruct_t<dd, CX>(cudaStream_t, View<dd>, View<const dd>, View<const dd>, const long long*);              \
+  template void lu_inverse_t<dd, CX>(cudaStream_t, View<dd>, View<const dd>, View<const dd>, const long long*);
+FB_RECON_INST_DD(false)
+FB_RECON_INST_DD(true)
+#undef FB_RECON_INST_DD
+#endif
 
 template <class R, bool CX>
 void permute_rows_t(cudaStream_t st, View<R> rhs, const long long* perm) {
@@ -267,6 +284,10 @@ template void permute_rows_t<double, false>(cudaStream_t, View<double>, const lo
 template void permute_rows_t<float, false>(cudaStream_t, View<float>, const long long*);
 template void permute_rows_t<double, true>(cudaStream_t, View<double>, const long long*);
 template void permute_rows_t<float, true>(cudaStream_t, View<float>, const long long*);
+#if defined(__CUDACC__)
+template void permute_rows_t<dd, false>(cudaStream_t, View<dd>, const long long*);
+template void permute_rows_t<dd, true>(cudaStream_t, View<dd>, const long long*);
+#endif
 
 template <class R, bool CX>
 void gather_2d_t(cudaStream_t st, View<R> out, View<const R> src, const long long* p, const long long* q) {

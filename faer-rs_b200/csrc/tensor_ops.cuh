@@ -2,10 +2,25 @@
 // are written once. f64 -> DMMA GEMM (gemm_f64.cu), f32 -> 3xTF32 GEMM (gemm_f32.cu), c64 / c32 on those (gemm_c64.cu,
 // gemm_c32.cu); triangular solves from trsm.cu and cplx.cu.
 #pragma once
+#include <type_traits>
+
 #include "gemm_f32.cuh"
 #include "linalg_f64.cuh"
 
 namespace fb {
+
+// ---- double-double kinds <dd, false> (fx128) and <dd, true> (cx128); dd.cuh, gemm_dd.cu, dd_factor.cu. Complex views are in
+// complex units on a dd* base. `alpha_im` is ignored by the real kind. ----
+struct dd;
+void gemm_dd(cudaStream_t st, View<dd> dst, int ds, int accum, View<const dd> lhs, int ls, bool conj_lhs, View<const dd> rhs, int rs,
+             bool conj_rhs, bool cx, dd alpha_re, dd alpha_im);
+void solve_lower_dd(cudaStream_t st, View<const dd> t, bool unit, bool conj, View<dd> rhs, bool cx);
+void solve_upper_dd(cudaStream_t st, View<const dd> t, bool unit, bool conj, View<dd> rhs, bool cx);
+// LLT / partial-pivoting LU drivers (dd_factor.cu); perm arrays: HOST int64 of A.nrows entries
+template <bool CX>
+LltResult llt_dd(cudaStream_t st, View<dd> A, dd delta, dd eps, size_t recursion_threshold, size_t block_size);
+template <bool CX>
+size_t lu_dd(cudaStream_t st, View<dd> A, size_t recursion_threshold, long long* perm_fwd, long long* perm_bwd);
 
 inline void gemm(cudaStream_t st, VD dst, int ds, int accum, VCD lhs, int ls, VCD rhs, int rs, double alpha) {
   gemm_f64(st, dst, ds, accum, lhs, ls, rhs, rs, alpha);
@@ -27,19 +42,22 @@ inline View<const T> cview(const View<T>& v) { return View<const T>{v.ptr, v.nro
 template <class R, bool CX>
 inline void gemm_t(cudaStream_t st, View<R> dst, int ds, int accum, View<const R> lhs, int ls, bool conj_lhs, View<const R> rhs,
                    int rs, bool conj_rhs, R alpha) {
-  if constexpr (!CX) gemm(st, dst, ds, accum, lhs, ls, rhs, rs, alpha);
+  if constexpr (std::is_same_v<R, dd>) gemm_dd(st, dst, ds, accum, lhs, ls, conj_lhs, rhs, rs, conj_rhs, CX, alpha, R(0));
+  else if constexpr (!CX) gemm(st, dst, ds, accum, lhs, ls, rhs, rs, alpha);
   else if constexpr (sizeof(R) == 8) gemm_c64(st, dst, ds, accum, lhs, ls, conj_lhs, rhs, rs, conj_rhs, alpha, 0.0);
   else gemm_c32(st, dst, ds, accum, lhs, ls, conj_lhs, rhs, rs, conj_rhs, alpha, 0.0f);
 }
 template <class R, bool CX>
 inline void solve_lower_t(cudaStream_t st, View<const R> t, bool unit, bool conj, View<R> rhs) {
-  if constexpr (!CX) solve_lower(st, t, unit, rhs);
+  if constexpr (std::is_same_v<R, dd>) solve_lower_dd(st, t, unit, conj, rhs, CX);
+  else if constexpr (!CX) solve_lower(st, t, unit, rhs);
   else if constexpr (sizeof(R) == 8) solve_lower_triangular_in_place_c64(st, t, unit, conj, rhs);
   else solve_lower_triangular_in_place_c32(st, t, unit, conj, rhs);
 }
 template <class R, bool CX>
 inline void solve_upper_t(cudaStream_t st, View<const R> t, bool unit, bool conj, View<R> rhs) {
-  if constexpr (!CX) solve_upper(st, t, unit, rhs);
+  if constexpr (std::is_same_v<R, dd>) solve_upper_dd(st, t, unit, conj, rhs, CX);
+  else if constexpr (!CX) solve_upper(st, t, unit, rhs);
   else if constexpr (sizeof(R) == 8) solve_upper_triangular_in_place_c64(st, t, unit, conj, rhs);
   else solve_upper_triangular_in_place_c32(st, t, unit, conj, rhs);
 }

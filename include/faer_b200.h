@@ -720,5 +720,6 @@ void libfaer_v0_23_partial_piv_lu_solve_transpose_in_place_u64_c32(struct FaerV0
 /* Bunch-Kaufman LBLT (lblt_*): declared in its own header */
 #include "faer_b200_lblt.h"
 #include "faer_b200_evd.h"
+#include "faer_b200_fx128.h"
 
 #endif /* LIBFAER_V0_24 */
