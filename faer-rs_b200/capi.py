@@ -300,7 +300,7 @@ def load() -> C.CDLL:
             f = getattr(lib, f"libfaer_v0_23_partial_piv_lu_factor_in_place_{it}_{suf}")
             f.argtypes = [MatMut, SliceMut, SliceMut, P, MemAlloc, PartialPivLuParams]
             f.restype = PartialPivLuStatus
-    for suf in ("f64", "f32", "c64", "c32"):
+    for suf in ("f64", "f32", "c64", "c32", "fx128", "cx128"):
         getattr(lib, f"libfaer_v0_23_QrParams_{suf}").argtypes = []
         getattr(lib, f"libfaer_v0_23_QrParams_{suf}").restype = QrParams
         f = getattr(lib, f"libfaer_v0_23_qr_recommended_block_size_{suf}")
@@ -463,6 +463,10 @@ def load() -> C.CDLL:
     lib.faer_b200_set_stream.restype = None
     lib.faer_b200_launch_count.argtypes = []
     lib.faer_b200_launch_count.restype = C.c_ulonglong
+    lib.faer_b200_launch_log_begin.argtypes = [C.c_void_p, C.c_size_t]
+    lib.faer_b200_launch_log_begin.restype = None
+    lib.faer_b200_launch_log_end.argtypes = []
+    lib.faer_b200_launch_log_end.restype = C.c_size_t
     lib.faer_b200_release_workspace.argtypes = []
     lib.faer_b200_release_workspace.restype = None
     lib.faer_b200_profile_begin.argtypes = []
@@ -613,6 +617,11 @@ def load() -> C.CDLL:
             "llt_inverse_scratch": ([C.c_size_t, P], Layout),
             "llt_inverse": ([MatMut, MatRef, P, MemAlloc], None),
             "PartialPivLuParams": ([], PartialPivLuParams),
+            # the rest of the QR family is in the QrParams loop above (include/faer_b200_fx128_qr.h)
+            "qr_reconstruct_scratch": ([C.c_size_t, C.c_size_t, C.c_size_t, P], Layout),
+            "qr_reconstruct": ([MatMut, MatRef, MatRef, MatRef, P, MemAlloc], None),
+            "qr_inverse_scratch": ([C.c_size_t, C.c_size_t, P], Layout),
+            "qr_inverse": ([MatMut, MatRef, MatRef, MatRef, P, MemAlloc], None),
         }
         for name in ("solve_triangular_lower", "solve_triangular_upper", "solve_unit_triangular_lower",
                      "solve_unit_triangular_upper"):

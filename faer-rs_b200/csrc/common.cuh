@@ -71,9 +71,27 @@ inline VCD cv(const VD& v) { return VCD{v.ptr, v.nrows, v.ncols, v.rs, v.cs}; }
     }                                                                              \
   } while (0)
 
-// every kernel launch of this library is counted (bench.py reports it as gpu_launches)
+// every kernel launch of this library is counted (bench.py reports it as gpu_launches). While a launch log is open
+// (faer_b200_launch_log_begin / _end), each counted launch also records the phase tag current when it was issued, so that a
+// profiler trace of the same launches can be split by phase (tools/time_fx128_qr.py).
 extern unsigned long long g_launch_count;
-inline void note_launch() { ++g_launch_count; }
+extern int g_launch_tag;
+extern signed char* g_launch_log;
+extern size_t g_launch_log_len, g_launch_log_cap;
+inline void note_launch() {
+  ++g_launch_count;
+  if (g_launch_log) {
+    if (g_launch_log_len < g_launch_log_cap) g_launch_log[g_launch_log_len] = (signed char)g_launch_tag;
+    ++g_launch_log_len;
+  }
+}
+enum LaunchPhase { LAUNCH_OTHER = 0, LAUNCH_PANEL = 1, LAUNCH_PRODUCT = 2, LAUNCH_TBUILD = 3 };
+// the phase of the launches issued while it is alive
+struct LaunchTag {
+  int prev;
+  explicit LaunchTag(LaunchPhase t) : prev(g_launch_tag) { g_launch_tag = t; }
+  ~LaunchTag() { g_launch_tag = prev; }
+};
 
 // ---- PTX helpers (device compilation only; the host build of the flat-map drivers, tools/emul/drivers_host.cpp, includes this
 // header through a plain C++ compiler) -----------------------------------------------------------

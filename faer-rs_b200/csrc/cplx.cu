@@ -1,6 +1,7 @@
 // c64 / c32 (complex<f64> / complex<f32>) triangular solves, Cholesky LLT, partial-pivoting LU and Householder QR (+ block-Householder
 // sequences): faer's recursions on the complex GEMMs (gemm_c64.cu, gemm_c32.cu) with small scalar complex leaf kernels, one source
-// templated over the real type R. (The comment blocks at the LU and QR sections cite their reference lines.)
+// templated over the real type R. (The comment blocks at the LU and QR sections cite their reference lines.) The blocked QR driver
+// and the Householder sequences are qr_blocked.cuh's, shared with the double-double kinds; this file supplies their c64 / c32 leaf.
 //
 // Reference:
 //   triangular_solve::solve_[unit_]{lower,upper}_triangular_in_place_with_conj   faer/src/linalg/triangular_solve.rs:220-604
@@ -19,6 +20,7 @@
 
 #include "gemm_f32.cuh"
 #include "linalg_f64.cuh"
+#include "qr_blocked.cuh"
 #include "runtime.cuh"
 
 namespace fb {
@@ -513,14 +515,11 @@ void lu_solve_transpose_in_place_cx(cudaStream_t st, View<const R> L, View<const
   permute_rows_cx<R>(st, rhs, perm_bwd);
 }
 
-// ---- Householder QR without pivoting for complex T (qr/no_pivoting/factor.rs:11-301; householder.rs:59-107, 132-272, 370-620,
-// 724-808) ---------------------------------------------------------------------------------------------------------------------
-// The reference's own structure: an unblocked kernel (one CTA) that carries the column-skipping rank logic, and the blocked
-// recursion above it on the host with every product on the complex GEMM; the recursion hands blocks of <= QR_LEAF columns to the
-// unblocked kernel whole (the reference's `m * n < blocking_threshold` branch), so one host read-back of the new row index per
-// leaf. Functional, not tuned: the panels run on a single SM.
+// ---- Householder QR without pivoting for complex T: the unblocked leaf (qr/no_pivoting/factor.rs:11-86; householder.rs:59-107).
+// One CTA carries the column-skipping rank logic; the blocked recursion above it is the shared driver of qr_blocked.cuh, which
+// hands it blocks of <= QR_LEAF columns (whole blocks under the reference's `m * n < blocking_threshold` branch). Functional, not
+// tuned: the panels run on a single SM.
 constexpr int QR_CT = 1024;
-constexpr int QR_LEAF = 16;
 
 template <class R>
 struct RealTraits;
@@ -687,36 +686,7 @@ __global__ void __launch_bounds__(QR_CT) qr_unblocked_cx_kernel(R* __restrict__ 
   if (tid == 0) out_row[0] = row;
 }
 
-// factor.rs:190-203: after a leaf produced `local` reflectors with sub-block size sbs, the s2 x s2 upper-triangular T blocks
-// sit in the first rows of H (view Hs: rows from `offset`, columns from `row`); block k moves down to rows [k, k + s2)
-template <class R>
-__global__ void qr_shift_tblocks_cx_kernel(R* __restrict__ Hs, i64 rs, i64 cs, int local, int sbs) {
-  for (int e = threadIdx.x; e < local * sbs; e += blockDim.x) {
-    const int col = e / sbs, i = e % sbs;
-    const int k = (col / sbs) * sbs, j = col - k;
-    if (k == 0 || i > j) continue;
-    cst(Hs, (i64)(k + i) * rs + (i64)col * cs, cld(Hs, (i64)i * rs + (i64)col * cs));
-  }
-}
-
-// factor.rs:283-299: columns >= rank of Q_coeff are zero with +inf on the block diagonals
-template <class R>
-__global__ void qr_finish_cx_kernel(R* __restrict__ H, i64 rs, i64 cs, int bs, int size, int rank) {
-  const i64 e = (i64)blockIdx.x * blockDim.x + threadIdx.x;
-  if (e >= (i64)bs * (size - rank)) return;
-  const int i = (int)(e % bs), j = rank + (int)(e / bs);
-  const bool diag = i == j - (j / bs) * bs;
-  cst(H, (i64)i * rs + (i64)j * cs, CxT<R>{diag ? R(INFINITY) : R(0), R(0)});
-}
-
-template <class R>
-struct QrCtx {
-  cudaStream_t st;
-  int* d_row;
-  R* tmp;  // block_size x ncols complex scratch of the block applies
-  i64 blocking_threshold;
-};
-
+// the reference's unblocked leaf on one CTA; one host read-back of the new row index per leaf
 template <class R>
 i64 qr_unblocked_cx(const QrCtx<R>& cx, View<R> A, View<R> Hrow, i64 row_start, i64 col_start) {
   if (!(row_start < std::min(Hrow.ncols, A.nrows) && col_start < A.ncols)) return row_start;
@@ -730,168 +700,17 @@ i64 qr_unblocked_cx(const QrCtx<R>& cx, View<R> A, View<R> Hrow, i64 row_start, 
   return h_row;
 }
 
-// upgrade_householder_factor (householder.rs:132-272): T = striu(V^H V), the diagonal (tau) kept
-template <class R>
-void upgrade_householder_factor_cx(cudaStream_t st, View<R> Tf, View<const R> V, i64 block_size, i64 prev_block_size) {
-  if (block_size == prev_block_size || Tf.nrows <= prev_block_size) return;
-  const i64 n = V.ncols;
-  const i64 block_count = (Tf.nrows + block_size - 1) / block_size;
-  if (block_count > 1) {
-    const i64 mid = block_count / 2;  // householder.rs:155-157 splits at the block COUNT
-    upgrade_householder_factor_cx<R>(st, csub(Tf, 0, 0, mid, mid), csub(V, 0, 0, V.nrows, mid), block_size, prev_block_size);
-    upgrade_householder_factor_cx<R>(st, csub(Tf, mid, mid, Tf.nrows - mid, Tf.ncols - mid),
-                                     csub(V, mid, mid, V.nrows - mid, V.ncols - mid), block_size, prev_block_size);
-    return;
-  }
-  if (prev_block_size < 8) {
-    View<const R> top = csub(V, 0, 0, n, n), bot = csub(V, n, 0, V.nrows - n, n);
-    cgemm(st, Tf, UNIT_UPPER, 0, top.t(), UNIT_UPPER, true, top, UNIT_LOWER, false, R(1), R(0));
-    if (bot.nrows > 0) cgemm(st, Tf, UNIT_UPPER, 1, bot.t(), RECT, true, bot, RECT, false, R(1), R(0));
-  } else {
-    const i64 prev_block_count = (Tf.nrows + prev_block_size - 1) / prev_block_size;
-    const i64 mid = (prev_block_count / 2) * prev_block_size;
-    View<R> tl = csub(Tf, 0, 0, mid, mid), tr = csub(Tf, 0, mid, mid, Tf.ncols - mid), br = csub(Tf, mid, mid, Tf.nrows - mid, Tf.ncols - mid);
-    View<const R> left = csub(V, 0, 0, V.nrows, mid), right = csub(V, mid, mid, V.nrows - mid, V.ncols - mid);
-    upgrade_householder_factor_cx<R>(st, tl, left, block_size, prev_block_size);
-    upgrade_householder_factor_cx<R>(st, br, right, block_size, prev_block_size);
-    View<const R> left2 = csub(left, mid, 0, left.nrows - mid, left.ncols);
-    const i64 row_mid = right.ncols;
-    View<const R> lt = csub(left2, 0, 0, row_mid, left2.ncols), lb = csub(left2, row_mid, 0, left2.nrows - row_mid, left2.ncols);
-    View<const R> rt = csub(right, 0, 0, row_mid, right.ncols), rb = csub(right, row_mid, 0, right.nrows - row_mid, right.ncols);
-    cgemm(st, tr, RECT, 0, lt.t(), RECT, true, rt, UNIT_LOWER, false, R(1), R(0));
-    if (lb.nrows > 0) cgemm(st, tr, RECT, 1, lb.t(), RECT, true, rb, RECT, false, R(1), R(0));
-  }
-}
-
-// apply_block_householder_on_the_left (householder.rs:370-620): M <- (I - V T^-1 V^H) M (forward = false) or
-// (I - V T^-H V^H) M (forward = true), conj_lhs conjugating V and T; tmp: N x K complex scratch
-template <class R>
-void apply_block_householder_left_cx(cudaStream_t st, View<const R> V, View<const R> Tf, bool conj_lhs, View<R> M, bool forward, R* tmpbuf) {
-  const i64 N = V.ncols, m = V.nrows, K = M.ncols;
-  if (N == 0 || K == 0) return;
-  View<R> tmp{tmpbuf, N, K, 1, N};
-  View<const R> Vt = csub(V, 0, 0, N, N), Vb = csub(V, N, 0, m - N, N);
-  View<R> top = csub(M, 0, 0, N, K), bot = csub(M, N, 0, m - N, K);
-  cgemm(st, tmp, RECT, 0, Vt.t(), UNIT_UPPER, !conj_lhs, View<const R>{top.ptr, N, K, top.rs, top.cs}, RECT, false, R(1), R(0));
-  if (m > N) cgemm(st, tmp, RECT, 1, Vb.t(), RECT, !conj_lhs, View<const R>{bot.ptr, m - N, K, bot.rs, bot.cs}, RECT, false, R(1), R(0));
-  if (forward) solve_lower_rec_cx<R>(st, Tf.t(), false, !conj_lhs, tmp);
-  else {
-    // upper = lower on the views with rows and columns reversed
-    View<const R> t{Tf.ptr + 2 * ((N - 1) * Tf.rs + (N - 1) * Tf.cs), N, N, -Tf.rs, -Tf.cs};
-    View<R> r{tmp.ptr + 2 * ((N - 1) * tmp.rs), N, K, -tmp.rs, tmp.cs};
-    solve_lower_rec_cx<R>(st, t, false, conj_lhs, r);
-  }
-  View<const R> ctmp{tmp.ptr, N, K, tmp.rs, tmp.cs};
-  cgemm(st, top, RECT, 1, Vt, UNIT_LOWER, conj_lhs, ctmp, RECT, false, R(-1), R(0));
-  if (m > N) cgemm(st, bot, RECT, 1, Vb, RECT, conj_lhs, ctmp, RECT, false, R(-1), R(0));
-}
-
-// qr_in_place_blocked (factor.rs:137-256)
-template <class R>
-i64 qr_blocked_cx(const QrCtx<R>& cx, View<R> A, View<R> H, i64 row_start, i64 col_start) {
-  const i64 m = A.nrows, n = A.ncols, size = std::min(m, n);
-  const i64 block_size0 = H.nrows;
-  if (block_size0 == 1) return qr_unblocked_cx<R>(cx, A, H, row_start, col_start);
-  const i64 sub_block_size0 = (block_size0 <= QR_LEAF || m * n < cx.blocking_threshold) ? 1 : block_size0 / 2;
-  i64 col = col_start, row = row_start;
-  while (row < size && col < n) {
-    const i64 block_size = std::min(block_size0, std::min(size - row, n - col));
-    const i64 sub_block_size = std::min(block_size, sub_block_size0);
-    const i64 start = row;
-    i64 offset = 0;
-    while (offset < block_size && col < n) {
-      const i64 bsz = std::min(n - col, block_size - offset);
-      const i64 sbs = std::min(bsz, sub_block_size);
-      const i64 new_row = qr_blocked_cx<R>(cx, csub(A, 0, 0, m, col + bsz), csub(H, offset, 0, sbs, H.ncols), row, col);
-      const i64 local = new_row - row;
-      if (local > 0) {
-        if (local > sbs) {
-          View<R> Hs = csub(H, offset, row, H.nrows - offset, local);
-          qr_shift_tblocks_cx_kernel<R><<<1, 256, 0, cx.st>>>(Hs.ptr, Hs.rs, Hs.cs, (int)local, (int)sbs);
-          FB_CUDA_CHECK(cudaGetLastError());
-          note_launch();
-        }
-        View<R> Arr = csub(A, row, row, m - row, local);
-        upgrade_householder_factor_cx<R>(cx.st, csub(H, offset, row, local, local), View<const R>{Arr.ptr, Arr.nrows, Arr.ncols, Arr.rs, Arr.cs},
-                                         local, sbs);
-        if (offset > 0) {
-          const i64 w = offset + local;
-          View<R> Hh = csub(H, 0, start, w, w);
-          View<R> Aa_ = csub(A, start, start, m - start, w);
-          View<const R> Aa{Aa_.ptr, Aa_.nrows, Aa_.ncols, Aa_.rs, Aa_.cs};
-          View<const R> A0 = csub(Aa, 0, 0, w, w), A1 = csub(Aa, w, 0, Aa.nrows - w, w);
-          cgemm(cx.st, Hh, UNIT_UPPER, 0, A0.t(), UNIT_UPPER, true, A0, UNIT_LOWER, false, R(1), R(0));
-          if (A1.nrows > 0) cgemm(cx.st, Hh, UNIT_UPPER, 1, A1.t(), RECT, true, A1, RECT, false, R(1), R(0));
-        }
-      }
-      View<R> below = csub(A, row, 0, m - row, n);
-      View<R> Q0_ = csub(below, 0, row, m - row, local);
-      View<R> A1 = csub(below, 0, col + bsz, m - row, n - (col + bsz));
-      View<R> Hq_ = csub(H, offset, row, local, local);
-      if (A1.ncols > 0 && local > 0)
-        apply_block_householder_left_cx<R>(cx.st, View<const R>{Q0_.ptr, Q0_.nrows, Q0_.ncols, Q0_.rs, Q0_.cs},
-                                           View<const R>{Hq_.ptr, Hq_.nrows, Hq_.ncols, Hq_.rs, Hq_.cs}, false, A1, true, cx.tmp);
-      offset += local;
-      row += local;
-      col += bsz;
-    }
-  }
-  return row;
-}
-
-// qr_in_place (factor.rs:258-301): returns the rank
-template <class R>
-i64 qr_in_place_cx(cudaStream_t st, View<R> A, View<R> Q_coeff, i64 blocking_threshold) {
-  const i64 m = A.nrows, n = A.ncols, size = std::min(m, n), bs = Q_coeff.nrows;
-  FB_ASSERT(bs > 0 && Q_coeff.ncols == size, "Q_coeff must be block_size x min(nrows, ncols)");
-  if (size == 0) return 0;
-  FB_ASSERT(m < (i64(1) << 31) && n < (i64(1) << 31), "complex QR dimensions limited to 2^31");
-  int* d_row = (int*)ws_alloc(sizeof(int));
-  R* tmp = (R*)ws_alloc((size_t)bs * (size_t)n * 2 * sizeof(R));
-  QrCtx<R> cx{st, d_row, tmp, blocking_threshold};
-  const i64 rank = qr_blocked_cx<R>(cx, A, Q_coeff, 0, 0);
-  if (rank < size) {
-    const i64 cnt = bs * (size - rank);
-    qr_finish_cx_kernel<R><<<(unsigned)((cnt + 255) / 256), 256, 0, st>>>(Q_coeff.ptr, Q_coeff.rs, Q_coeff.cs, (int)bs, (int)size, (int)rank);
-    FB_CUDA_CHECK(cudaGetLastError());
-    note_launch();
-  }
-  FB_CUDA_CHECK(cudaStreamSynchronize(st));
-  ws_free(tmp);
-  ws_free(d_row);
-  return rank;
-}
-
-// apply_block_householder_sequence_[transpose_]on_the_left_in_place_with_conj (householder.rs:724-808): rhs <- Q rhs or Q^H rhs
-// (with conj: the conjugated Q), Q given by its basis (unit-lower trapezoid) and block_size x size factor
-template <class R>
-void apply_householder_sequence_left_cx(cudaStream_t st, View<const R> basis, View<const R> factor, bool conj, View<R> rhs, bool transpose) {
-  const i64 bs = factor.nrows, size = factor.ncols, m = basis.nrows, K = rhs.ncols;
-  FB_ASSERT(bs > 0 && size == std::min(basis.nrows, basis.ncols) && rhs.nrows == m, "Householder sequence shape mismatch");
-  if (size == 0 || K == 0) return;
-  R* tmp = (R*)ws_alloc((size_t)bs * (size_t)K * 2 * sizeof(R));
-  if (transpose) {
-    // householder.rs:768-808: blocks in ascending order, each through transpose_on_the_left = conj composed with Yes, forward
-    for (i64 j = 0; j < size;) {
-      const i64 b = std::min(bs, size - j);
-      apply_block_householder_left_cx<R>(st, csub(basis, j, j, m - j, b), csub(factor, 0, j, b, b), !conj, csub(rhs, j, 0, m - j, K), true, tmp);
-      j += b;
-    }
-  } else {
-    // householder.rs:724-765: blocks in descending order (the last block may be short)
-    i64 j = size, b = size % bs ? size % bs : bs;
-    while (j > 0) {
-      const i64 jp = j - b;
-      apply_block_householder_left_cx<R>(st, csub(basis, jp, jp, m - jp, b), csub(factor, 0, jp, b, b), conj, csub(rhs, jp, 0, m - jp, K), false, tmp);
-      j = jp;
-      b = bs;
-    }
-  }
-  FB_CUDA_CHECK(cudaStreamSynchronize(st));
-  ws_free(tmp);
-}
-
 }  // namespace
+
+// the leaves of the blocked driver (qr_blocked.cuh) for c64 / c32
+template <>
+i64 qr_unblocked_t<double, true>(const QrCtx<double>& cx, View<double> A, View<double> Hrow, i64 row_start, i64 col_start) {
+  return qr_unblocked_cx<double>(cx, A, Hrow, row_start, col_start);
+}
+template <>
+i64 qr_unblocked_t<float, true>(const QrCtx<float>& cx, View<float> A, View<float> Hrow, i64 row_start, i64 col_start) {
+  return qr_unblocked_cx<float>(cx, A, Hrow, row_start, col_start);
+}
 
 // ---- exported entry points (linalg_f64.cuh / gemm_f32.cuh) ------------------------------------------------------------------
 #define FB_CPLX_EXPORTS(SUF, R)                                                                                                   \
@@ -916,11 +735,11 @@ void apply_householder_sequence_left_cx(cudaStream_t st, View<const R> basis, Vi
     lu_solve_transpose_in_place_cx<R>(st, L, U, conj, perm_bwd, rhs);                                                            \
   }                                                                                                                               \
   i64 qr_in_place_##SUF(cudaStream_t st, View<R> A, View<R> Q_coeff, i64 blocking_threshold) {                                   \
-    return qr_in_place_cx<R>(st, A, Q_coeff, blocking_threshold);                                                                \
+    return qr_in_place_t<R, true>(st, A, Q_coeff, blocking_threshold);                                                           \
   }                                                                                                                               \
   void apply_householder_sequence_left_##SUF(cudaStream_t st, View<const R> basis, View<const R> factor, bool conj, View<R> rhs, \
                                              bool transpose) {                                                                    \
-    apply_householder_sequence_left_cx<R>(st, basis, factor, conj, rhs, transpose);                                               \
+    apply_householder_sequence_left_t<R, true>(st, basis, factor, conj, rhs, transpose);                                            \
   }
 FB_CPLX_EXPORTS(c64, double)
 FB_CPLX_EXPORTS(c32, float)
@@ -928,7 +747,7 @@ FB_CPLX_EXPORTS(c32, float)
 
 template <class R>
 void householder_build_t_cx(cudaStream_t st, View<const R> V, View<R> Tf) {
-  upgrade_householder_factor_cx<R>(st, Tf, V, Tf.nrows, 1);
+  upgrade_householder_factor_t<R, true>(st, Tf, V, Tf.nrows, 1);
 }
 template void householder_build_t_cx<double>(cudaStream_t, View<const double>, View<double>);
 template void householder_build_t_cx<float>(cudaStream_t, View<const float>, View<float>);

@@ -138,6 +138,32 @@ DD_HD dd sqrt(dd a) {
 // faer's mul_add for fx128: add(mul(a, b), acc)
 DD_HD dd dd_mul_add(dd a, dd b, dd acc) { return a * b + acc; }
 
+// fx128's real-field constants (faer-traits/src/lib.rs, the RealField impl for fx128): MIN_POSITIVE = (f64::MIN_POSITIVE, 0),
+// sqrt_min_positive / sqrt_max_positive = sqrt(MIN_POSITIVE) / sqrt(recip(MIN_POSITIVE)), eps = Quad::EPSILON * 8 (both limbs
+// scaled). Quad::EPSILON comes from the `qd` crate, whose source is not part of the reference; its value is the double-double
+// unit roundoff 2^-104, so eps = 2^-101 here. The rank test is its only user and only its magnitude matters there.
+DD_HD dd dd_min_positive() { return dd(2.2250738585072014e-308); }
+DD_HD dd dd_sqrt_min_positive() { return sqrt(dd_min_positive()); }
+DD_HD dd dd_sqrt_max_positive() { return sqrt(dd_recip(dd_min_positive())); }
+DD_HD dd dd_eps() { return dd(0x1p-101); }
+DD_HD dd dd_infinity() { return dd(INFINITY); }
+
+// faer's abs_impl (faer-traits/src/lib.rs:337-352) in dd arithmetic: sqrt(re^2 + im^2) with the operands scaled by
+// sqrt_min_positive or sqrt_max_positive when they are large or small. It is the modulus of a cx128 value and, as
+// math_utils::hypot, fx128's hypot (lib.rs:163-165).
+DD_HD dd dd_abs_impl(dd re, dd im) {
+  const dd small = dd_sqrt_min_positive(), big = dd_sqrt_max_positive(), one(1.0);
+  const dd ra = fabs(re), ia = fabs(im);
+  if (ra > big || ia > big) {
+    const dd r = re * small, i = im * small;
+    return sqrt(r * r + i * i) * big;
+  }
+  if (ra > one || ia > one) return sqrt(re * re + im * im);
+  const dd r = re * big, i = im * big;
+  return sqrt(r * r + i * i) * small;
+}
+DD_HD dd dd_hypot(dd a, dd b) { return dd_abs_impl(a, b); }
+
 #if defined(__CUDACC__)
 __device__ __forceinline__ dd __ldcg(const dd* p) {
   const double2 v = ::__ldcg((const double2*)p);
@@ -157,6 +183,8 @@ DD_HD cdd operator*(cdd a, cdd b) { return cdd{a.re * b.re - a.im * b.im, a.re *
 DD_HD cdd cdd_scale(cdd a, dd s) { return cdd{a.re * s, a.im * s}; }
 // |re| + |im| (faer's abs1 for cx128)
 DD_HD dd cdd_abs1(cdd a) { return fabs(a.re) + fabs(a.im); }
+// the modulus (faer's abs for cx128)
+DD_HD dd cdd_abs(cdd a) { return dd_abs_impl(a.re, a.im); }
 // faer's recip_impl (faer-traits/src/lib.rs:353-383) in dd arithmetic; small / big are fx128's sqrt_min_positive /
 // sqrt_max_positive, the square roots of MIN_POSITIVE = (f64::MIN_POSITIVE, 0) and of its reciprocal
 DD_HD cdd cdd_recip(cdd x) {
@@ -179,6 +207,20 @@ DD_HD cdd cdd_recip(cdd x) {
   const dd r = re * big, i = im * big;
   const dd inv = dd_recip(r * r + i * i);
   return cdd{(r * inv) * big, (-i * inv) * big};
+}
+// 1 / x with x first scaled by an exact power of two that brings its larger part near 1. cdd_recip's scaling by sqrt_max_positive
+// leaves |x|^-2 near MIN_POSITIVE when |x| <= 1 (and near the overflow threshold for |x| below about 2^-970), where the low limb
+// falls into the subnormals and the result keeps only about 53 bits; here both limbs stay normal wherever the result can hold
+// them. Zero, subnormal (the scale factor would overflow), non-finite and NaN inputs go to cdd_recip.
+DD_HD cdd cdd_recip_scaled(cdd x) {
+  const double mx = fmax(fabs(x.re.hi), fabs(x.im.hi));
+  if (!(mx >= 0x1p-1022 && mx <= 0x1.fffffffffffffp+1023) || isnan(x.re.lo) || isnan(x.im.lo)) return cdd_recip(x);
+  int e;
+  frexp(mx, &e);
+  const dd s(ldexp(1.0, -e));
+  const dd re = x.re * s, im = x.im * s;
+  const dd inv = dd_recip(re * re + im * im) * s;
+  return cdd{re * inv, -(im * inv)};
 }
 
 }  // namespace fb

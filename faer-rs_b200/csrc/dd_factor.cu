@@ -65,7 +65,8 @@ __global__ void __launch_bounds__(128) dd_trsm_leaf_kernel(View<const dd> L, boo
     if (k > i) continue;
     cdd v = dl_ld<CX>(L.ptr, i * L.rs + k * L.cs);
     if (conj) v = cdd_conj(v);
-    if (k == i) v = unit ? cdd{dd(1.0), dd(0.0)} : dl_recip<CX>(v);
+    // the complex reciprocal keeps both limbs for diagonals of modulus <= 1 (dd.cuh, cdd_recip_scaled)
+    if (k == i) v = unit ? cdd{dd(1.0), dd(0.0)} : (CX ? cdd_recip_scaled(v) : dl_recip<CX>(v));
     else v = -v;
     Ls[i][k] = v;
   }

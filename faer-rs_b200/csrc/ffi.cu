@@ -65,9 +65,6 @@ FaerV0_24_QrStatus qr_entry(FaerV0_24_MatMut A, FaerV0_24_MatMut Q) {
   }
   return out;
 }
-inline FaerV0_24_MatMut transposed(FaerV0_24_MatMut m) {
-  return FaerV0_24_MatMut{m.ptr, m.ncols, m.nrows, m.col_stride, m.row_stride};
-}
 template <class T>
 void householder_seq_entry(FaerV0_24_MatRef basis, FaerV0_24_MatRef factor, FaerV0_24_MatMut rhs, bool transpose) {
   FB_ENTRY();
@@ -1409,6 +1406,17 @@ int faer_b200_device_count(void) {
 }
 void faer_b200_set_stream(void* cuda_stream) { std::lock_guard<std::recursive_mutex> lock(entry_mutex()); set_current_stream((cudaStream_t)cuda_stream); }
 unsigned long long faer_b200_launch_count(void) { return g_launch_count; }
+void faer_b200_launch_log_begin(signed char* tags, size_t capacity) {
+  std::lock_guard<std::recursive_mutex> lock(entry_mutex());
+  g_launch_log = tags;
+  g_launch_log_cap = capacity;
+  g_launch_log_len = 0;
+}
+size_t faer_b200_launch_log_end(void) {
+  std::lock_guard<std::recursive_mutex> lock(entry_mutex());
+  g_launch_log = nullptr;
+  return g_launch_log_len;
+}
 void faer_b200_release_workspace(void) { std::lock_guard<std::recursive_mutex> lock(entry_mutex()); ws_release_all(); }
 void faer_b200_profile_begin(void) { std::lock_guard<std::recursive_mutex> lock(entry_mutex()); profile_begin(); }
 void faer_b200_profile_end(double* flops, double* ms, unsigned long long* count) {

@@ -93,5 +93,9 @@ static inline FaerV0_24_Layout layout_and(FaerV0_24_Layout a, size_t b_bytes) {
   const size_t off = (a.len_bytes + 63) / 64 * 64;
   return FaerV0_24_Layout{off + b_bytes, al};
 }
+// the transposed view: "on the right" is the transposed sequence on the left of it (householder.rs:813-854)
+inline FaerV0_24_MatMut transposed(FaerV0_24_MatMut m) {
+  return FaerV0_24_MatMut{m.ptr, m.ncols, m.nrows, m.col_stride, m.row_stride};
+}
 
 }  // namespace fb

@@ -1,7 +1,8 @@
 // extern "C" boundary of the double-double kinds (include/faer_b200_fx128.h): fx128 = <dd, false>, cx128 = <dd, true>. Same
 // conventions as ffi.cu / ffi_types.cu (by-value PODs, synchronous on return, abort() on precondition violations, host buffers
 // staged, device buffers used in place, `Par` ignored). Drivers: gemm_dd.cu, dd_factor.cu and the <dd, CX> instantiations of the
-// reconstruct_types.cu compositions. Scratch sizes are the f64 formulas with 16 / 32-byte elements.
+// reconstruct_types.cu compositions, qr_dd.cu for the Householder QR (include/faer_b200_fx128_qr.h). Scratch sizes are the f64
+// formulas (c64 for the QR family) with 16 / 32-byte elements.
 #include "../../include/faer_b200.h"
 #include "dd.cuh"
 #include "ffi_common.cuh"
@@ -9,6 +10,7 @@
 #include "tensor_ops.cuh"
 
 #include <cstring>
+#include <memory>
 #include <vector>
 
 using namespace fb;
@@ -174,6 +176,71 @@ void lu_recon_dd(FaerV0_24_MatMut A, FaerV0_24_MatRef L, FaerV0_24_MatRef U, Fae
   finish_all(st, {&a, &l, &u});
 }
 
+// QR factor (qr/no_pivoting/factor.rs:258-301): returns the rank
+template <bool CX>
+FaerV0_24_QrStatus qr_factor_dd(FaerV0_24_MatMut A, FaerV0_24_MatMut Q, FaerV0_24_QrParams params) {
+  FB_ENTRY();
+  cudaStream_t st = current_stream();
+  const size_t size = A.nrows < A.ncols ? A.nrows : A.ncols;
+  FB_ASSERT(Q.nrows > 0 && Q.ncols == size, "Q_coeff must be block_size x min(nrows, ncols)");
+  StagedMat a = stage<CX>(A, true, st), q = stage<CX>(Q, true, st);
+  const i64 rank = qr_dd<CX>(st, a.view<dd>(), q.view<dd>(), (i64)params.blocking_threshold);
+  finish_all(st, {&a, &q});
+  FaerV0_24_QrStatus out;
+  memset(&out, 0, sizeof(out));
+  out.tag = FaerV0_24_QrStatus_Ok;
+  out.ok.rank = (size_t)rank;
+  return out;
+}
+
+// rhs <- Q rhs (transpose = false) or Q^H rhs (true), Q conjugated for cx128 under Conj::Yes (householder.rs:724-808)
+template <bool CX>
+void householder_seq_dd(FaerV0_24_MatRef basis, FaerV0_24_MatRef factor, FaerV0_24_Conj conj, FaerV0_24_MatMut rhs, bool transpose) {
+  FB_ENTRY();
+  cudaStream_t st = current_stream();
+  StagedMat b = stage<CX>(basis, st), f = stage<CX>(factor, st), r = stage<CX>(rhs, true, st);
+  householder_sequence_dd<CX>(st, b.view<const dd>(), f.view<const dd>(), CX && conj == FaerV0_24_Conj_Yes, r.view<dd>(), transpose);
+  finish_all(st, {&b, &f, &r});
+}
+
+// qr/no_pivoting/solve.rs:38-176. mode 0: least squares (m >= n), 1: square solve, 2: transpose solve. R may alias Q_basis (the
+// packed factorization), which is then staged once.
+template <bool CX>
+void qr_solve_dd(FaerV0_24_MatRef Qb, FaerV0_24_MatRef Qc, FaerV0_24_MatRef Rm, FaerV0_24_Conj A_conj, FaerV0_24_MatMut rhs, int mode) {
+  FB_ENTRY();
+  cudaStream_t st = current_stream();
+  const size_t m = Qb.nrows, n = Qb.ncols, size = m < n ? m : n;
+  FB_ASSERT(Qc.nrows > 0 && rhs.nrows == m && m >= n && Qc.ncols == size && Rm.nrows >= size && Rm.ncols == n, "QR solve shape mismatch");
+  if (mode != 0) FB_ASSERT(m == n && Rm.nrows == n, "QR solve: the factorization must be square");
+  if (size == 0 || rhs.ncols == 0) return;
+  const bool cj = CX && A_conj == FaerV0_24_Conj_Yes;
+  StagedMat b = stage<CX>(Qb, st), f = stage<CX>(Qc, st), r = stage<CX>(rhs, true, st);
+  const bool alias = Rm.ptr == Qb.ptr && Rm.row_stride == Qb.row_stride && Rm.col_stride == Qb.col_stride;
+  std::unique_ptr<StagedMat> rr;
+  if (!alias) rr.reset(new StagedMat(Rm.ptr, (i64)size, (i64)n, (i64)Rm.row_stride, (i64)Rm.col_stride, es<CX>(), true, false, st));
+  const View<const dd> Rv = sub_t<dd, CX>(alias ? b.view<const dd>() : rr->view<const dd>(), 0, 0, (i64)size, (i64)n);
+  const View<dd> x = r.view<dd>();
+  if (mode == 2) {
+    solve_lower_t<dd, CX>(st, Rv.t(), false, cj, x);                                           // op(R)^T y = rhs
+    householder_sequence_dd<CX>(st, b.view<const dd>(), f.view<const dd>(), CX && !cj, x, false);  // the forward sequence, conj composed with Yes
+  } else {
+    householder_sequence_dd<CX>(st, b.view<const dd>(), f.view<const dd>(), CX && !cj, x, true);   // op(Q)^H rhs
+    solve_upper_t<dd, CX>(st, Rv, false, cj, sub_t<dd, CX>(x, 0, 0, (i64)size, x.ncols));
+  }
+  finish_all(st, {&b, &f, &r});
+  if (rr) rr->finish();
+}
+
+template <bool CX>
+void qr_recon_dd(FaerV0_24_MatMut A, FaerV0_24_MatRef Qb, FaerV0_24_MatRef Qc, FaerV0_24_MatRef Rm, bool inverse) {
+  FB_ENTRY();
+  cudaStream_t st = current_stream();
+  StagedMat a = stage<CX>(A, false, st), b = stage<CX>(Qb, st), f = stage<CX>(Qc, st), r = stage<CX>(Rm, st);
+  if (inverse) qr_inverse_t<dd, CX>(st, a.view<dd>(), b.view<const dd>(), f.view<const dd>(), r.view<const dd>());
+  else qr_reconstruct_t<dd, CX>(st, a.view<dd>(), b.view<const dd>(), f.view<const dd>(), r.view<const dd>());
+  finish_all(st, {&a, &b, &f, &r});
+}
+
 }  // namespace
 
 extern "C" {
@@ -325,5 +392,117 @@ FB_DD_LU_FFI(u64, 8, fx128, false)
 FB_DD_LU_FFI(u32, 4, cx128, true)
 FB_DD_LU_FFI(u64, 8, cx128, true)
 #undef FB_DD_LU_FFI
+
+// ---- Householder QR, block-Householder sequences and the QR solves: the c64 entries' semantics and scratch formulas ----
+#define FB_DD_QR_FFI(SUF, CX)                                                                                                    \
+  FaerV0_24_QrParams libfaer_v0_23_QrParams_##SUF(void) { return FaerV0_24_QrParams{48 * 48, 192 * 256}; }                      \
+  size_t libfaer_v0_23_qr_recommended_block_size_##SUF(size_t nrows, size_t ncols) {                                            \
+    return (size_t)qr_recommended_block_size((i64)nrows, (i64)ncols);                                                           \
+  }                                                                                                                             \
+  FaerV0_24_Layout libfaer_v0_23_qr_factor_in_place_scratch_##SUF(size_t nrows, size_t ncols, size_t block_size,                \
+                                                                  FaerV0_24_Par par, FaerV0_24_QrParams params) {               \
+    (void)nrows; (void)par; (void)params;                                                                                       \
+    return FaerV0_24_Layout{block_size * ncols * es<CX>(), 64};                                                                 \
+  }                                                                                                                             \
+  FaerV0_24_QrStatus libfaer_v0_23_qr_factor_in_place_##SUF(FaerV0_24_MatMut A, FaerV0_24_MatMut Q_coeff, FaerV0_24_Par par,    \
+                                                            FaerV0_24_MemAlloc mem, FaerV0_24_QrParams params) {                \
+    (void)par; (void)mem;                                                                                                       \
+    return qr_factor_dd<CX>(A, Q_coeff, params);                                                                                \
+  }                                                                                                                             \
+  FaerV0_24_Layout libfaer_v0_23_apply_householder_on_the_left_scratch_##SUF(size_t dim, size_t block_size, size_t rhs_ncols) { \
+    (void)dim;                                                                                                                  \
+    return FaerV0_24_Layout{block_size * rhs_ncols * es<CX>(), 64};                                                             \
+  }                                                                                                                             \
+  FaerV0_24_Layout libfaer_v0_23_apply_householder_transpose_on_the_left_scratch_##SUF(size_t dim, size_t block_size,           \
+                                                                                        size_t rhs_ncols) {                     \
+    (void)dim;                                                                                                                  \
+    return FaerV0_24_Layout{block_size * rhs_ncols * es<CX>(), 64};                                                             \
+  }                                                                                                                             \
+  void libfaer_v0_23_apply_householder_on_the_left_##SUF(FaerV0_24_MatRef basis, FaerV0_24_MatRef factor, FaerV0_24_Conj conj,  \
+                                                         FaerV0_24_MatMut rhs, FaerV0_24_Par par, FaerV0_24_MemAlloc mem) {     \
+    (void)par; (void)mem;                                                                                                       \
+    householder_seq_dd<CX>(basis, factor, conj, rhs, false);                                                                    \
+  }                                                                                                                             \
+  void libfaer_v0_23_apply_householder_transpose_on_the_left_##SUF(FaerV0_24_MatRef basis, FaerV0_24_MatRef factor,             \
+                                                                   FaerV0_24_Conj conj, FaerV0_24_MatMut rhs,                   \
+                                                                   FaerV0_24_Par par, FaerV0_24_MemAlloc mem) {                 \
+    (void)par; (void)mem;                                                                                                       \
+    householder_seq_dd<CX>(basis, factor, conj, rhs, true);                                                                     \
+  }                                                                                                                             \
+  /* on the right = the transposed sequence on the left of the transposed view, and vice versa (householder.rs:813-854) */     \
+  FaerV0_24_Layout libfaer_v0_23_apply_householder_on_the_right_scratch_##SUF(size_t dim, size_t block_size, size_t lhs_nrows) { \
+    (void)dim;                                                                                                                  \
+    return FaerV0_24_Layout{block_size * lhs_nrows * es<CX>(), 64};                                                             \
+  }                                                                                                                             \
+  FaerV0_24_Layout libfaer_v0_23_apply_householder_transpose_on_the_right_scratch_##SUF(size_t dim, size_t block_size,          \
+                                                                                         size_t lhs_nrows) {                    \
+    (void)dim;                                                                                                                  \
+    return FaerV0_24_Layout{block_size * lhs_nrows * es<CX>(), 64};                                                             \
+  }                                                                                                                             \
+  void libfaer_v0_23_apply_householder_on_the_right_##SUF(FaerV0_24_MatRef basis, FaerV0_24_MatRef factor, FaerV0_24_Conj conj, \
+                                                          FaerV0_24_MatMut lhs, FaerV0_24_Par par, FaerV0_24_MemAlloc mem) {    \
+    (void)par; (void)mem;                                                                                                       \
+    householder_seq_dd<CX>(basis, factor, conj, transposed(lhs), true);                                                         \
+  }                                                                                                                             \
+  void libfaer_v0_23_apply_householder_transpose_on_the_right_##SUF(FaerV0_24_MatRef basis, FaerV0_24_MatRef factor,            \
+                                                                    FaerV0_24_Conj conj, FaerV0_24_MatMut lhs,                  \
+                                                                    FaerV0_24_Par par, FaerV0_24_MemAlloc mem) {                \
+    (void)par; (void)mem;                                                                                                       \
+    householder_seq_dd<CX>(basis, factor, conj, transposed(lhs), false);                                                        \
+  }                                                                                                                             \
+  FaerV0_24_Layout libfaer_v0_23_qr_solve_lstsq_in_place_scratch_##SUF(size_t nrows, size_t ncols, size_t block_size,           \
+                                                                       size_t rhs_ncols, FaerV0_24_Par par) {                   \
+    (void)nrows; (void)ncols; (void)par;                                                                                        \
+    return FaerV0_24_Layout{block_size * rhs_ncols * es<CX>(), 64};                                                             \
+  }                                                                                                                             \
+  FaerV0_24_Layout libfaer_v0_23_qr_solve_in_place_scratch_##SUF(size_t dim, size_t block_size, size_t rhs_ncols,               \
+                                                                 FaerV0_24_Par par) {                                           \
+    (void)dim; (void)par;                                                                                                       \
+    return FaerV0_24_Layout{block_size * rhs_ncols * es<CX>(), 64};                                                             \
+  }                                                                                                                             \
+  FaerV0_24_Layout libfaer_v0_23_qr_solve_transpose_in_place_scratch_##SUF(size_t dim, size_t block_size,                       \
+                                                                           size_t rhs_ncols, FaerV0_24_Par par) {               \
+    (void)dim; (void)par;                                                                                                       \
+    return FaerV0_24_Layout{block_size * rhs_ncols * es<CX>(), 64};                                                             \
+  }                                                                                                                             \
+  void libfaer_v0_23_qr_solve_lstsq_in_place_##SUF(FaerV0_24_MatRef Q_basis, FaerV0_24_MatRef Q_coeff, FaerV0_24_MatRef R,      \
+                                                   FaerV0_24_Conj A_conj, FaerV0_24_MatMut rhs, FaerV0_24_Par par,              \
+                                                   FaerV0_24_MemAlloc mem) {                                                    \
+    (void)par; (void)mem;                                                                                                       \
+    qr_solve_dd<CX>(Q_basis, Q_coeff, R, A_conj, rhs, 0);                                                                       \
+  }                                                                                                                             \
+  void libfaer_v0_23_qr_solve_in_place_##SUF(FaerV0_24_MatRef Q_basis, FaerV0_24_MatRef Q_coeff, FaerV0_24_MatRef R,            \
+                                             FaerV0_24_Conj A_conj, FaerV0_24_MatMut rhs, FaerV0_24_Par par,                    \
+                                             FaerV0_24_MemAlloc mem) {                                                          \
+    (void)par; (void)mem;                                                                                                       \
+    qr_solve_dd<CX>(Q_basis, Q_coeff, R, A_conj, rhs, 1);                                                                       \
+  }                                                                                                                             \
+  void libfaer_v0_23_qr_solve_transpose_in_place_##SUF(FaerV0_24_MatRef Q_basis, FaerV0_24_MatRef Q_coeff, FaerV0_24_MatRef R,  \
+                                                       FaerV0_24_Conj A_conj, FaerV0_24_MatMut rhs, FaerV0_24_Par par,          \
+                                                       FaerV0_24_MemAlloc mem) {                                                \
+    (void)par; (void)mem;                                                                                                       \
+    qr_solve_dd<CX>(Q_basis, Q_coeff, R, A_conj, rhs, 2);                                                                       \
+  }                                                                                                                             \
+  FaerV0_24_Layout libfaer_v0_23_qr_reconstruct_scratch_##SUF(size_t nrows, size_t ncols, size_t block_size, FaerV0_24_Par par) { \
+    (void)nrows; (void)par;                                                                                                     \
+    return FaerV0_24_Layout{block_size * ncols * es<CX>(), 64};                                                                 \
+  }                                                                                                                             \
+  void libfaer_v0_23_qr_reconstruct_##SUF(FaerV0_24_MatMut A, FaerV0_24_MatRef Q_basis, FaerV0_24_MatRef Q_coeff,               \
+                                          FaerV0_24_MatRef R, FaerV0_24_Par par, FaerV0_24_MemAlloc mem) {                      \
+    (void)par; (void)mem;                                                                                                       \
+    qr_recon_dd<CX>(A, Q_basis, Q_coeff, R, false);                                                                             \
+  }                                                                                                                             \
+  FaerV0_24_Layout libfaer_v0_23_qr_inverse_scratch_##SUF(size_t dim, size_t block_size, FaerV0_24_Par par) {                   \
+    (void)par;                                                                                                                  \
+    return FaerV0_24_Layout{block_size * dim * es<CX>(), 64};                                                                   \
+  }                                                                                                                             \
+  void libfaer_v0_23_qr_inverse_##SUF(FaerV0_24_MatMut A, FaerV0_24_MatRef Q_basis, FaerV0_24_MatRef Q_coeff, FaerV0_24_MatRef R, \
+                                      FaerV0_24_Par par, FaerV0_24_MemAlloc mem) {                                              \
+    (void)par; (void)mem;                                                                                                       \
+    qr_recon_dd<CX>(A, Q_basis, Q_coeff, R, true);                                                                              \
+  }
+FB_DD_QR_FFI(fx128, false)
+FB_DD_QR_FFI(cx128, true)
+#undef FB_DD_QR_FFI
 
 }  // extern "C"

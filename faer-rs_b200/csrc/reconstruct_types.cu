@@ -136,7 +136,9 @@ struct Kind {
 // (householder.rs:768-808 as qr/no_pivoting/solve.rs:60-67 calls it)
 template <class R, bool CX>
 void rt_hh_seq(cudaStream_t st, View<const R> b, View<const R> f, View<R> rhs, bool adjoint) {
-  if constexpr (!CX) {
+  if constexpr (std::is_same_v<R, dd>) {
+    householder_sequence_dd<CX>(st, b, f, adjoint, rhs, adjoint);
+  } else if constexpr (!CX) {
     if (adjoint) apply_block_householder_sequence_transpose_on_the_left<R>(st, b, f, rhs);
     else apply_block_householder_sequence_on_the_left<R>(st, b, f, rhs);
   } else if constexpr (sizeof(R) == 8) {
@@ -265,12 +267,14 @@ FB_RECON_INST(float, false)
 FB_RECON_INST(double, true)
 FB_RECON_INST(float, true)
 #undef FB_RECON_INST
-#if defined(__CUDACC__)  // double-double: the LLT and LU compositions (there is no dd Householder QR)
+#if defined(__CUDACC__)  // double-double: the LLT, LU and QR compositions
 #define FB_RECON_INST_DD(CX)                                                                                                     \
   template void llt_reconstruct_t<dd, CX>(cudaStream_t, View<dd>, View<const dd>);                                               \
   template void llt_inverse_t<dd, CX>(cudaStream_t, View<dd>, View<const dd>);                                                   \
   template void lu_reconstruct_t<dd, CX>(cudaStream_t, View<dd>, View<const dd>, View<const dd>, const long long*);              \
-  template void lu_inverse_t<dd, CX>(cudaStream_t, View<dd>, View<const dd>, View<const dd>, const long long*);
+  template void lu_inverse_t<dd, CX>(cudaStream_t, View<dd>, View<const dd>, View<const dd>, const long long*);                  \
+  template void qr_reconstruct_t<dd, CX>(cudaStream_t, View<dd>, View<const dd>, View<const dd>, View<const dd>);                \
+  template void qr_inverse_t<dd, CX>(cudaStream_t, View<dd>, View<const dd>, View<const dd>, View<const dd>);
 FB_RECON_INST_DD(false)
 FB_RECON_INST_DD(true)
 #undef FB_RECON_INST_DD

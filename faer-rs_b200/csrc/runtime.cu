@@ -8,6 +8,9 @@
 namespace fb {
 
 unsigned long long g_launch_count = 0;
+int g_launch_tag = LAUNCH_OTHER;
+signed char* g_launch_log = nullptr;
+size_t g_launch_log_len = 0, g_launch_log_cap = 0;
 
 namespace {
 cudaStream_t g_stream = nullptr;

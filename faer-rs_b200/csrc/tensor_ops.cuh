@@ -21,6 +21,12 @@ template <bool CX>
 LltResult llt_dd(cudaStream_t st, View<dd> A, dd delta, dd eps, size_t recursion_threshold, size_t block_size);
 template <bool CX>
 size_t lu_dd(cudaStream_t st, View<dd> A, size_t recursion_threshold, long long* perm_fwd, long long* perm_bwd);
+// Householder QR (qr/no_pivoting/factor.rs:258-301; returns the rank) and block-Householder sequences (householder.rs:724-808:
+// rhs <- Q rhs, or Q^H rhs with `transpose`; `conj` conjugates Q) (qr_dd.cu)
+template <bool CX>
+i64 qr_dd(cudaStream_t st, View<dd> A, View<dd> Q_coeff, i64 blocking_threshold);
+template <bool CX>
+void householder_sequence_dd(cudaStream_t st, View<const dd> basis, View<const dd> factor, bool conj, View<dd> rhs, bool transpose);
 
 inline void gemm(cudaStream_t st, VD dst, int ds, int accum, VCD lhs, int ls, VCD rhs, int rs, double alpha) {
   gemm_f64(st, dst, ds, accum, lhs, ls, rhs, rs, alpha);

@@ -564,6 +564,10 @@ int faer_b200_device_count(void);
 void faer_b200_set_stream(void *cuda_stream);
 /* Number of kernels this library has launched since load (for bench.py's gpu_launches). */
 unsigned long long faer_b200_launch_count(void);
+/* Launch-phase log: between begin and end, each launch of this library stores its phase in tags[i] (i < capacity; 0 other,
+ * 1 dd QR panel, 2 Householder products, 3 T-factor builds); end() returns the number of launches, which may exceed capacity. */
+void faer_b200_launch_log_begin(signed char *tags, size_t capacity);
+size_t faer_b200_launch_log_end(void);
 /* Free the cached device workspace. */
 void faer_b200_release_workspace(void);
 /* Per-launch timing of the dominant kernel (the DMMA GEMM): between begin and end every GEMM launch is bracketed by
@@ -721,5 +725,6 @@ void libfaer_v0_23_partial_piv_lu_solve_transpose_in_place_u64_c32(struct FaerV0
 #include "faer_b200_lblt.h"
 #include "faer_b200_evd.h"
 #include "faer_b200_fx128.h"
+#include "faer_b200_fx128_qr.h"
 
 #endif /* LIBFAER_V0_24 */

@@ -23,6 +23,12 @@ extern "C" int dd_host_op(int op, const double* a, const double* b, double* out,
       case 8: r = dd(x > y ? 1.0 : 0.0); break;
       case 9: r = dd(x >= y ? 1.0 : 0.0); break;
       case 10: r = dd(x == y ? 1.0 : 0.0); break;
+      case 11: r = fb::dd_hypot(x, y); break;                   // fx128 hypot
+      case 12: r = fb::cdd_abs(fb::cdd{x, y}); break;           // |x + i y| of cx128
+      case 13: r = fb::dd_sqrt_min_positive(); break;
+      case 14: r = fb::dd_sqrt_max_positive(); break;
+      case 15: r = fb::cdd_recip_scaled(fb::cdd{x, y}).re; break;   // 1 / (x + i y) of cx128
+      case 16: r = fb::cdd_recip_scaled(fb::cdd{x, y}).im; break;
       default: return -1;
     }
     out[2 * i] = r.hi;

@@ -13,6 +13,9 @@ static long long g_guard_errors = 0, g_live_blocks = 0;
 namespace fb {
 
 unsigned long long g_launch_count = 0;
+int g_launch_tag = 0;
+signed char* g_launch_log = nullptr;
+size_t g_launch_log_len = 0, g_launch_log_cap = 0;
 
 // ---- checking allocator ----
 namespace {
