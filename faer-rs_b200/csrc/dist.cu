@@ -13,7 +13,7 @@
 // The same block-column drivers run the large single-GPU factorizations (P = 1, no communicator). Three single-GPU
 // refinements live here as well:
 //   * SM partitioning with CUDA green contexts (`ensure_green_streams`): the LU panel chain gets its own SMs, the
-//     trailing updates an urgent and a bulk stream on the rest (`lu_local_partitioned_f64`; LLT variant opt-in);
+//     trailing updates an urgent and a bulk stream on the rest (`lu_local_partitioned_f64`);
 //   * on one GPU the LLT trailing update of a step is ONE structured launch instead of one per block column;
 //   * host-resident matrices are streamed through the LLT (`llt_host_pipelined_f64`): uploads, factorization and
 //     downloads of finished panels overlap.
@@ -47,6 +47,7 @@ ncclComm_t g_comm = nullptr;
 int g_rank = 0, g_nranks = 1;
 cudaStream_t g_panel_stream = nullptr;  // high priority: panel factorization + broadcast
 cudaStream_t g_main_stream = nullptr;   // trailing updates
+cudaStream_t g_side_stream = nullptr;   // high priority: the LLT's look-ahead column update below its diagonal block
 
 bool load_nccl() {
   if (g_nccl.handle) return true;
@@ -109,6 +110,7 @@ static void ensure_streams() {
   FB_CUDA_CHECK(cudaDeviceGetStreamPriorityRange(&lo, &hi));
   FB_CUDA_CHECK(cudaStreamCreateWithPriority(&g_panel_stream, cudaStreamNonBlocking, hi));
   FB_CUDA_CHECK(cudaStreamCreateWithPriority(&g_main_stream, cudaStreamNonBlocking, lo));
+  FB_CUDA_CHECK(cudaStreamCreateWithPriority(&g_side_stream, cudaStreamNonBlocking, hi));
 }
 
 // ---- SM partitioning for the single-GPU look-ahead (CUDA green contexts) ------------------------------------------
@@ -372,116 +374,9 @@ void dist_finalize() {
   }
   if (g_panel_stream) cudaStreamDestroy(g_panel_stream), g_panel_stream = nullptr;
   if (g_main_stream) cudaStreamDestroy(g_main_stream), g_main_stream = nullptr;
+  if (g_side_stream) cudaStreamDestroy(g_side_stream), g_side_stream = nullptr;
   g_rank = 0;
   g_nranks = 1;
-}
-
-// -----------------------------------------------------------------------------------------------------------------
-// Single-GPU right-looking block-column LLT on a partitioned GPU (green contexts, see above). Three streams:
-//   sp  panel partition            : Cholesky of the diagonal block (the serial potf2 / small-TRSM / small-SYRK chain)
-//   su  update partition, urgent   : update of block column k+1 with panel k, then the panel solve below the diagonal
-//   sm  update partition, bulk     : update of block columns k+2.. with panel k (column k+2 first: it is the next urgent one)
-// Per-element update order is k = 0, 1, ... as in every other driver, so the factor is bit-identical to theirs.
-// -----------------------------------------------------------------------------------------------------------------
-static LltResult llt_local_partitioned_f64(double* A, i64 ld, i64 n, i64 nb, double reg_delta, double reg_eps) {
-  LltResult res{true, 0, 0};
-  cudaStream_t sp = g_green_panel, su = g_green_urgent, sm = g_green_main;
-  const bool trace = getenv("FAER_B200_TRACE") != nullptr;  // dev aid: print the event timeline of the three streams
-  const unsigned evf = trace ? cudaEventDefault : cudaEventDisableTiming;
-  cudaEvent_t ev_start;
-  FB_CUDA_CHECK(cudaEventCreateWithFlags(&ev_start, evf));
-  FB_CUDA_CHECK(cudaEventRecord(ev_start, current_stream()));
-  FB_CUDA_CHECK(cudaStreamWaitEvent(sp, ev_start, 0));
-  FB_CUDA_CHECK(cudaStreamWaitEvent(su, ev_start, 0));
-  FB_CUDA_CHECK(cudaStreamWaitEvent(sm, ev_start, 0));
-  const i64 nblk = nblocks(n, nb);
-  long long* d_info = (long long*)ws_alloc(4 * sizeof(long long));
-  long long h_info[2] = {-1, 0};
-  FB_CUDA_CHECK(cudaMemcpyAsync(d_info, h_info, sizeof(h_info), cudaMemcpyHostToDevice, sp));
-  std::vector<cudaEvent_t> ev_panel((size_t)nblk), ev_diag((size_t)nblk), ev_ready((size_t)nblk), ev_first((size_t)nblk);
-  for (i64 k = 0; k < nblk; ++k) {
-    FB_CUDA_CHECK(cudaEventCreateWithFlags(&ev_panel[(size_t)k], evf));
-    FB_CUDA_CHECK(cudaEventCreateWithFlags(&ev_diag[(size_t)k], evf));
-    FB_CUDA_CHECK(cudaEventCreateWithFlags(&ev_ready[(size_t)k], evf));
-    FB_CUDA_CHECK(cudaEventCreateWithFlags(&ev_first[(size_t)k], evf));
-  }
-  auto factor_diag = [&](i64 k) {  // on sp
-    const i64 k0 = k * nb, kb = std::min(nb, n - k0);
-    VD diag{A + k0 * ld + k0, kb, kb, 1, ld};
-    llt_cholesky_device_f64(sp, diag, reg_delta, reg_eps, d_info, k0);
-    FB_CUDA_CHECK(cudaEventRecord(ev_diag[(size_t)k], sp));
-  };
-  auto solve_below = [&](i64 k) {  // on su
-    const i64 k0 = k * nb, kb = std::min(nb, n - k0), rows = n - k0;
-    FB_CUDA_CHECK(cudaStreamWaitEvent(su, ev_diag[(size_t)k], 0));
-    if (rows > kb) {
-      VD diag{A + k0 * ld + k0, kb, kb, 1, ld};
-      VD below{A + k0 * ld + k0 + kb, rows - kb, kb, 1, ld};
-      solve_lower_triangular_in_place_f64(su, cv(diag), false, below.t());
-    }
-    FB_CUDA_CHECK(cudaEventRecord(ev_panel[(size_t)k], su));
-  };
-  auto update_block_col = [&](cudaStream_t st, i64 k, i64 j) {
-    const i64 k0 = k * nb, kb = std::min(nb, n - k0);
-    const i64 j0 = j * nb, jb = std::min(nb, n - j0);
-    VCD Wj{A + k0 * ld + j0, jb, kb, 1, ld};  // rows of block j in panel k
-    VD djj{A + j0 * ld + j0, jb, jb, 1, ld};
-    gemm_f64(st, djj, TRI_LOWER, 1, Wj, RECT, Wj.t(), RECT, -1.0);
-    const i64 below = n - j0 - jb;
-    if (below > 0) {
-      VCD Wb{A + k0 * ld + j0 + jb, below, kb, 1, ld};
-      VD dbj{A + j0 * ld + j0 + jb, below, jb, 1, ld};
-      gemm_f64(st, dbj, 1, Wb, Wj.t(), -1.0);
-    }
-  };
-  factor_diag(0);
-  solve_below(0);
-  for (i64 k = 0; k < nblk; ++k) {
-    const i64 kn = k + 1;
-    if (kn < nblk) {
-      // su already holds ev_panel[k] in stream order; column kn has its updates 0..k-1 once bulk step k-1 did its first column
-      if (k >= 1) FB_CUDA_CHECK(cudaStreamWaitEvent(su, ev_first[(size_t)(k - 1)], 0));
-      update_block_col(su, k, kn);
-      FB_CUDA_CHECK(cudaEventRecord(ev_ready[(size_t)kn], su));
-      FB_CUDA_CHECK(cudaStreamWaitEvent(sp, ev_ready[(size_t)kn], 0));
-      factor_diag(kn);
-      solve_below(kn);
-    }
-    FB_CUDA_CHECK(cudaStreamWaitEvent(sm, ev_panel[(size_t)k], 0));
-    for (i64 j = k + 2; j < nblk; ++j) {
-      update_block_col(sm, k, j);
-      if (j == k + 2) FB_CUDA_CHECK(cudaEventRecord(ev_first[(size_t)k], sm));
-    }
-  }
-  FB_CUDA_CHECK(cudaMemcpyAsync(h_info, d_info, sizeof(h_info), cudaMemcpyDeviceToHost, sp));
-  FB_CUDA_CHECK(cudaStreamSynchronize(sp));
-  FB_CUDA_CHECK(cudaStreamSynchronize(su));
-  FB_CUDA_CHECK(cudaStreamSynchronize(sm));
-  if (trace) {
-    auto at = [&](cudaEvent_t e) {
-      float ms = 0.f;
-      return cudaEventElapsedTime(&ms, ev_start, e) == cudaSuccess ? ms : -1.f;
-    };
-    fprintf(stderr, "LLT n=%lld nb=%lld timeline (ms since start): k: col-ready diag-done panel-done bulk-first\n", n, nb);
-    for (i64 k = 0; k < nblk; ++k)
-      fprintf(stderr, "  %3lld: %8.3f %8.3f %8.3f %8.3f\n", k, k ? at(ev_ready[(size_t)k]) : 0.f, at(ev_diag[(size_t)k]),
-              at(ev_panel[(size_t)k]), k + 2 < nblk ? at(ev_first[(size_t)k]) : -1.f);
-  }
-  for (i64 k = 0; k < nblk; ++k) {
-    cudaEventDestroy(ev_panel[(size_t)k]);
-    cudaEventDestroy(ev_diag[(size_t)k]);
-    cudaEventDestroy(ev_ready[(size_t)k]);
-    cudaEventDestroy(ev_first[(size_t)k]);
-  }
-  cudaEventDestroy(ev_start);
-  ws_free(d_info);
-  if (h_info[0] >= 0) {
-    res.ok = false;
-    res.non_positive_pivot_index = (size_t)h_info[0];
-  } else {
-    res.dynamic_regularization_count = (size_t)h_info[1];
-  }
-  return res;
 }
 
 // -----------------------------------------------------------------------------------------------------------------
@@ -503,17 +398,26 @@ LltResult dist_llt_f64(double* A_local, i64 ld, i64 n, i64 nb, double reg_delta,
   FB_ASSERT(nb > 0 && nb % 2 == 0, "block size must be positive and even");
   if (lookahead) ensure_streams();
   LltHostPipe* pipe = (P == 1 && lookahead) ? g_llt_pipe : nullptr;  // host-resident matrix streamed through (see below)
-  // (the LLT chain kernels are small enough to slip in between GEMM CTAs, so the partitioned LLT driver stays opt-in:
-  // FAER_B200_GREEN_LLT=1)
-  if (!pipe && lookahead && P == 1 && getenv("FAER_B200_GREEN_LLT") && ensure_green_streams())
-    return llt_local_partitioned_f64(A_local, ld, n, nb, reg_delta, reg_eps);
+  // Single GPU: the chain (sp, high priority) and the bulk update (sm) share every SM. A wide bulk CTA fills its SM (384
+  // threads x 168 registers, ~225 KB of shared memory), so a chain kernel starts only as bulk CTAs end; that is why the
+  // bulk CTAs are short-lived. Giving the chain SMs of its own (green-context partitions) measured 1.2-2.5x slower at
+  // n = 16384: potf2 takes ~95 us per launch alone as in the step, while the panel solve, the column update and the bulk
+  // lose SMs (profiles/r13_llt_chain_*.json, H100 SXM at 700 W).
   cudaStream_t sp = lookahead ? g_panel_stream : current_stream();
   cudaStream_t sm = lookahead ? g_main_stream : current_stream();
   const bool two_streams = sp != sm && lookahead;
   if (!two_streams) sm = sp;
+  // Single GPU: the look-ahead update of block column k+1 is split. Its diagonal block is updated on sp, and the part
+  // below it on the side stream ss, where it runs beside the diagonal block's factorization (potf2 alone is ~95 us per
+  // 128 columns); sp joins ss before the panel solve. Same kernels on the same operands, so the factor is unchanged.
+  // In the 128-wide tail the chain, not the trailing update, sets the step time.
+  cudaStream_t ss = (two_streams && P == 1) ? g_side_stream : sp;
   // order after whatever the caller enqueued on the current stream
-  cudaEvent_t ev_start;
+  cudaEvent_t ev_start, ev_fork, ev_join;
+  bool join_pending = false;
   FB_CUDA_CHECK(cudaEventCreateWithFlags(&ev_start, cudaEventDisableTiming));
+  FB_CUDA_CHECK(cudaEventCreateWithFlags(&ev_fork, cudaEventDisableTiming));
+  FB_CUDA_CHECK(cudaEventCreateWithFlags(&ev_join, cudaEventDisableTiming));
   FB_CUDA_CHECK(cudaEventRecord(ev_start, current_stream()));
   FB_CUDA_CHECK(cudaStreamWaitEvent(sp, ev_start, 0));
   if (two_streams) FB_CUDA_CHECK(cudaStreamWaitEvent(sm, ev_start, 0));
@@ -541,19 +445,35 @@ LltResult dist_llt_f64(double* A_local, i64 ld, i64 n, i64 nb, double reg_delta,
     const i64 k0 = b0[(size_t)k], kb = b0[(size_t)k + 1] - k0, rows = n - k0;
     const int owner = (int)(k % P);
     double* Wk = W[k & 1];
+    cudaStream_t packed_on = sp;  // the stream that completes W_k
     if (k >= 2) FB_CUDA_CHECK(cudaStreamWaitEvent(sp, ev_used[(size_t)(k - 2)], 0));  // buffer reuse
     if (owner == me) {
       double* pk = A_local + col_off(k) * ld + k0;
       VD diag{pk, kb, kb, 1, ld};
       llt_cholesky_device_f64(sp, diag, reg_delta, reg_eps, d_info, k0);
+      if (join_pending) {  // the look-ahead update below the diagonal block (ss)
+        FB_CUDA_CHECK(cudaStreamWaitEvent(sp, ev_join, 0));
+        join_pending = false;
+      }
       if (rows > kb) {
         VD below{pk + kb, rows - kb, kb, 1, ld};
         solve_lower_triangular_in_place_f64(sp, cv(diag), false, below.t());
       }
-      pack(sp, Wk, pk, ld, rows, kb);
+      // split look-ahead (ss != sp): sp packs only the rows the next diagonal-block update reads, ss the rest (the rows
+      // its own update below that block and the trailing update read)
+      const i64 head = (ss != sp && k + 1 < nblk) ? b0[(size_t)k + 2] - k0 : rows;
+      FB_CUDA_CHECK(cudaMemcpy2DAsync(Wk, (size_t)rows * 8, pk, (size_t)ld * 8, (size_t)head * 8, (size_t)kb,
+                                      cudaMemcpyDeviceToDevice, sp));
+      if (head < rows) {
+        FB_CUDA_CHECK(cudaEventRecord(ev_fork, sp));
+        FB_CUDA_CHECK(cudaStreamWaitEvent(ss, ev_fork, 0));
+        FB_CUDA_CHECK(cudaMemcpy2DAsync(Wk + head, (size_t)rows * 8, pk + head, (size_t)ld * 8, (size_t)(rows - head) * 8,
+                                        (size_t)kb, cudaMemcpyDeviceToDevice, ss));
+        packed_on = ss;
+      }
     }
     if (P > 1) FB_NCCL_CHECK(g_nccl.Broadcast(Wk, Wk, (size_t)rows * kb, ncclDouble, owner, g_comm, sp));
-    FB_CUDA_CHECK(cudaEventRecord(ev_bcast[(size_t)k], sp));
+    FB_CUDA_CHECK(cudaEventRecord(ev_bcast[(size_t)k], packed_on));
     if (pipe) {  // block column k is final: send it home while the factorization goes on
       FB_CUDA_CHECK(cudaStreamWaitEvent(pipe->s_d2h, ev_bcast[(size_t)k], 0));
       FB_CUDA_CHECK(cudaMemcpy2DAsync(pipe->host + k0 * pipe->host_ld + k0, (size_t)pipe->host_ld * 8,
@@ -562,8 +482,9 @@ LltResult dist_llt_f64(double* A_local, i64 ld, i64 n, i64 nb, double reg_delta,
     }
   };
 
-  auto update_block_col = [&](cudaStream_t st, i64 k, i64 j) {
-    // block column j (> k, owned by me) -= W_k[rows >= j0] * W_k[rows of block j]^T
+  auto update_block_col = [&](cudaStream_t st, i64 k, i64 j, cudaStream_t st_below) {
+    // block column j (> k, owned by me) -= W_k[rows >= j0] * W_k[rows of block j]^T; the part below the diagonal block
+    // on st_below (ordered after st's work so far, joined by the panel solve of block j)
     if (pipe && k == 0) FB_CUDA_CHECK(cudaStreamWaitEvent(st, pipe->up[(size_t)j], 0));  // first touch of column j
     const i64 k0 = b0[(size_t)k], kb = b0[(size_t)k + 1] - k0, rows_k = n - k0;
     const i64 j0 = b0[(size_t)j], jb = b0[(size_t)j + 1] - j0;
@@ -571,12 +492,20 @@ LltResult dist_llt_f64(double* A_local, i64 ld, i64 n, i64 nb, double reg_delta,
     double* pj = A_local + col_off(j) * ld + j0;
     VCD Wj{Wk + (j0 - k0), jb, kb, 1, rows_k};                       // rows of block j in the panel
     VD djj{pj, jb, jb, 1, ld};
-    gemm_f64(st, djj, TRI_LOWER, 1, Wj, RECT, Wj.t(), RECT, -1.0);    // diagonal block: lower triangle only
     const i64 below = n - j0 - jb;
+    if (below > 0 && st_below != st) {
+      FB_CUDA_CHECK(cudaEventRecord(ev_fork, st));
+      FB_CUDA_CHECK(cudaStreamWaitEvent(st_below, ev_fork, 0));
+    }
+    gemm_f64(st, djj, TRI_LOWER, 1, Wj, RECT, Wj.t(), RECT, -1.0);    // diagonal block: lower triangle only
     if (below > 0) {
       VCD Wb{Wk + (j0 - k0) + jb, below, kb, 1, rows_k};
       VD dbj{pj + jb, below, jb, 1, ld};
-      gemm_f64(st, dbj, 1, Wb, Wj.t(), -1.0);
+      gemm_f64(st_below, dbj, 1, Wb, Wj.t(), -1.0);
+      if (st_below != st) {
+        FB_CUDA_CHECK(cudaEventRecord(ev_join, st_below));
+        join_pending = true;
+      }
     }
   };
 
@@ -591,7 +520,7 @@ LltResult dist_llt_f64(double* A_local, i64 ld, i64 n, i64 nb, double reg_delta,
         // look-ahead: bring block column k+1 up to date first (on the panel stream), then factor + broadcast it
         // block column k+1 has received updates 0..k-1 on sm; order sp after them
         if (two_streams && k >= 1) FB_CUDA_CHECK(cudaStreamWaitEvent(sp, ev_used[(size_t)(k - 1)], 0));
-        update_block_col(sp, k, kn);
+        update_block_col(sp, k, kn, ss);
       }
       factor_and_bcast(kn);
     }
@@ -604,7 +533,7 @@ LltResult dist_llt_f64(double* A_local, i64 ld, i64 n, i64 nb, double reg_delta,
       gemm_f64(sm, dst, TRI_LOWER, 1, Wr, RECT, Wr.t(), RECT, -1.0);
     } else {
       for (i64 j = k + 2; j < nblk; ++j)
-        if ((int)(j % P) == me) update_block_col(sm, k, j);
+        if ((int)(j % P) == me) update_block_col(sm, k, j, sm);
     }
     FB_CUDA_CHECK(cudaEventRecord(ev_used[(size_t)k], sm));
   }
@@ -620,6 +549,8 @@ LltResult dist_llt_f64(double* A_local, i64 ld, i64 n, i64 nb, double reg_delta,
     cudaEventDestroy(ev_used[(size_t)k]);
   }
   cudaEventDestroy(ev_start);
+  cudaEventDestroy(ev_fork);
+  cudaEventDestroy(ev_join);
   ws_free(d_info);
   ws_free(W[1]);
   ws_free(W[0]);

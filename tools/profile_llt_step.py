@@ -1,7 +1,10 @@
 """Per-kernel breakdown of ONE f64 LLT step of the headline workload (n = 16384, bench.py's input and call) with
 torch.profiler: device time per kernel name, summed over the step; how much of the step no kernel covers (exposed gaps);
 per CUDA stream (the look-ahead driver's bulk-update stream and its high-priority panel stream), the busy time and the
-kernel time per name, and the wall time during which only the panel stream is busy; and the largest trailing update (lower-triangular n = 16128, k = 256) timed on its own with CUDA events.
+kernel time per name, and the wall time during which only the panel stream is busy; the same split per block tier (the
+512-wide head, the 256 tier and the 128 tail, told apart by their potf2 launches: 4, 2 and 1 per block column), with the
+chain kernels' mean time per launch; and the largest trailing update (lower-triangular n = 16128, k = 256) timed on its
+own with CUDA events. The FAER_B200_* variables in the environment select the schedule as in the library.
 usage: python tools/profile_llt_step.py [out_dir]   (writes out_dir/llt_step_profile.json)"""
 import json
 import os
@@ -113,6 +116,43 @@ if by_gemm:
             "kernels": dict(sorted(streams[s]["kernels"].items(), key=lambda kv: -kv[1]["ms"]))}
     per_stream["only_panel_busy_ms"] = only_panel / 1e3
 
+    # per tier: potf2 launches in time order; the head has 16 block columns of 4, the 256 tier 8 of 2, the tail 1 each
+    kev = [ev for ev in trace.get("traceEvents", []) if ev.get("cat") == "kernel"]
+    tr0, tr1 = min(ev["ts"] for ev in kev), max(ev["ts"] + ev["dur"] for ev in kev)  # the trace's own clock
+    potf2 = sorted(ev["ts"] for ev in kev if "potf2" in ev["name"])
+    edges = [tr0, potf2[64], potf2[80], tr1] if len(potf2) == 128 else None
+
+    def clip(iv, lo, hi):
+        return [(max(s, lo), min(e, hi)) for s, e in iv if e > lo and s < hi]
+
+    def length(iv):
+        return sum(e - s for s, e in union(iv))
+
+    def minus(a, b):  # length of union(a) not covered by union(b)
+        return length(a) - length([(max(s, bs), min(e, be)) for s, e in union(a) for bs, be in union(b)
+                                   if min(e, be) > max(s, bs)])
+
+    if edges:
+        tiers = {}
+        all_iv = [iv for s in streams for iv in streams[s]["iv"]]
+        for name, lo, hi in (("512", edges[0], edges[1]), ("256", edges[1], edges[2]), ("128_tail", edges[2], edges[3])):
+            chain = {}
+            for s in by_gemm[1:]:
+                for ev in trace["traceEvents"]:
+                    if ev.get("cat") != "kernel" or ev.get("args", {}).get("stream") != s or not lo <= ev["ts"] < hi:
+                        continue
+                    m = re.search(r"(\w+_kernel)\b", ev["name"])
+                    d = chain.setdefault(m.group(1) if m else ev["name"][:80], {"ms": 0.0, "launches": 0})
+                    d["ms"] += ev["dur"] / 1e3
+                    d["launches"] += 1
+            for d in chain.values():
+                d["us_per_launch"] = d["ms"] * 1e3 / d["launches"]
+            tiers[name] = {"wall_ms": (hi - lo) / 1e3,
+                           "only_panel_busy_ms": minus(clip(panel, lo, hi), clip(bulk, lo, hi)) / 1e3,
+                           "no_kernel_ms": (hi - lo - length(clip(all_iv, lo, hi))) / 1e3,
+                           "panel_kernels": dict(sorted(chain.items(), key=lambda kv: -kv[1]["ms"]))}
+        per_stream["tiers"] = tiers
+
 # the largest trailing update on its own: dst(lower, 16128^2) -= P P^T, P 16128 x 256 (the shape of the first block step)
 m, k = n - 256, 256
 P = torch.randn((k, m), dtype=torch.float64, device=dev).T
@@ -124,7 +164,8 @@ for _ in range(10):
     e0 = torch.cuda.Event(enable_timing=True); e1 = torch.cuda.Event(enable_timing=True)
     e0.record(); f(); e1.record(); torch.cuda.synchronize()
     best = min(best, e0.elapsed_time(e1))
-res = {"n": n, "step_ms": (t1 - t0) / 1e3, "kernel_busy_ms": busy / 1e3, "exposed_gap_ms": (t1 - t0 - busy) / 1e3,
+res = {"n": n, "env": {k: v for k, v in os.environ.items() if k.startswith("FAER_B200_")},
+       "step_ms": (t1 - t0) / 1e3, "kernel_busy_ms": busy / 1e3, "exposed_gap_ms": (t1 - t0 - busy) / 1e3,
        "kernels": per, "streams": per_stream,
        "largest_update": {"m": m, "k": k, "ms": best, "tflops": m * (m + 1.0) * k / (best * 1e-3) / 1e12}}
 print(json.dumps(res, indent=1))
