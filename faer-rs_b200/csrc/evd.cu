@@ -6,7 +6,8 @@
 // This file is the VALUES-ONLY path (U passed with no columns); with eigenvectors the entry point goes to svd_vectors.cu
 // (divide and conquer of the tridiagonal, tridiag_dc.cu, + the Householder back-transform). Any n (tridiag.cu keeps its
 // per-CTA vectors in global memory above n = 8192).
-// STATUS: validated on hardware (tests/test_gpu_zz8_self_adjoint_eigenvalues.py, tests/test_gpu_zz11_evd_svd_vectors.py); tridiag_ev.cuh is also
+// STATUS: validated on hardware (tests/test_gpu_zz8_self_adjoint_eigenvalues.py, tests/test_gpu_zz11_evd_svd_vectors.py,
+// tests/test_gpu_zz24_spectral_exact.py); tridiag_ev.cuh is also
 // checked on the CPU (the same header compiled for the host, tests/test_tridiag_ev_cpu.py).
 #include "runtime.cuh"
 #include "tensor_ops.cuh"

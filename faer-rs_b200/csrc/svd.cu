@@ -7,7 +7,8 @@
 // through bidiag_svd (QR iteration / divide and conquer); here they are located by Sturm counts — same values to
 // n * eps * sigma_max, the small ones to high relative accuracy; (2) this file is the VALUES-ONLY path (U and V passed with no
 // columns); with vectors the entry point goes to svd_vectors.cu (divide and conquer + back-transforms).
-// STATUS: validated on hardware (tests/test_gpu_zz7_singular_values.py and the fixture files of tests/test_gpu_zz11_evd_svd_vectors.py);
+// STATUS: validated on hardware (tests/test_gpu_zz7_singular_values.py and the fixture files of tests/test_gpu_zz11_evd_svd_vectors.py,
+// exact spectra in tests/test_gpu_zz24_spectral_exact.py);
 // bidiag_sv.cuh is also checked on the CPU (the same header compiled for the host, tests/test_bidiag_sv_cpu.py).
 #include "bidiag_sv.cuh"
 #include "runtime.cuh"

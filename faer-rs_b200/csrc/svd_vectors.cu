@@ -26,6 +26,8 @@
 //     the signs go into U_B, and a final stable ordering makes S non-increasing as the reference promises.
 //   Cost at n = 8192: eigensolver on 2n (4/3 (2n)^3 flop of GEMM), two QRs and two applications of their Q to the
 //   identity: ~16 n^3 flop on the DMMA path, a fraction of the 1 s the HBM-bound bidiagonalization takes.
+// STATUS: validated on hardware (tests/test_gpu_zz11_evd_svd_vectors.py; exact spectra, rank-deficient and repeated singular
+// values, and sizes past 8192 rows in tests/test_gpu_zz24_spectral_exact.py).
 #include <algorithm>
 
 #include "bidiag_sv.cuh"

@@ -23,7 +23,8 @@
 //       Q_new[lo:mid, lo:hi] = Q1 * W[0:s1, :],  Q_new[mid:hi, lo:hi] = Q2 * W[s1:, :]   — two DMMA GEMMs per merge
 //     (4/3 n^3 flop over all levels; deflation is not exploited to shrink them).
 // Eigenvalues come out ascending, eigenvectors orthogonal to working precision whatever the clustering (tests:
-// tests/test_tridiag_dc_cpu.py on the CPU harness, tests/test_gpu_zz11_evd_svd.py on the device).
+// tests/test_tridiag_dc_cpu.py on the CPU harness, tests/test_gpu_zz11_evd_svd_vectors.py and
+// tests/test_gpu_zz24_spectral_exact.py on the device).
 #include <algorithm>
 #include <vector>
 
