@@ -342,6 +342,7 @@ def load() -> C.CDLL:
         f = getattr(lib, f"libfaer_v0_23_svd_{suf}")
         f.argtypes = [MatRef, MatMut, VecMut, MatMut, P, MemAlloc, SvdParams]
         f.restype = SvdStatus
+    for suf in ("f64", "f32", "c64", "c32", "fx128", "cx128"):
         getattr(lib, f"libfaer_v0_23_TridiagParams_{suf}").argtypes = []
         getattr(lib, f"libfaer_v0_23_TridiagParams_{suf}").restype = TridiagParams
         getattr(lib, f"libfaer_v0_23_SelfAdjointEvdParams_{suf}").argtypes = []

@@ -85,7 +85,7 @@ inline void note_launch() {
     ++g_launch_log_len;
   }
 }
-enum LaunchPhase { LAUNCH_OTHER = 0, LAUNCH_PANEL = 1, LAUNCH_PRODUCT = 2, LAUNCH_TBUILD = 3 };
+enum LaunchPhase { LAUNCH_OTHER = 0, LAUNCH_PANEL = 1, LAUNCH_PRODUCT = 2, LAUNCH_TBUILD = 3, LAUNCH_SOLVE = 4 };
 // the phase of the launches issued while it is alive
 struct LaunchTag {
   int prev;

@@ -4,7 +4,8 @@
 //
 // Operations (faer-traits/src/lib.rs, the fx128 impl; the algorithms are Dekker's and Knuth's):
 //   add      two_sum of the high parts, the low parts added to the error, one quick_two_sum ("sloppy" add; faer's add_estimate)
-//   sub      add(a, -b), as faer's SIMD loops do (DESIGN.md §7: sub_accurate below is only used inside sqrt's Newton step)
+//   sub      add(a, -b), as faer's SIMD loops do (DESIGN.md §7: sub_accurate below is used inside sqrt's Newton step and for the
+//            differences the dd divide and conquer needs to relative accuracy, evd_dd.cu)
 //   mul      FMA two_prod of the high parts, the cross products added to the error, one quick_two_sum
 //   div      one correction step from hi / hi;  recip: 0 when |hi| is infinite, 1 / x otherwise
 //   sqrt     one Newton step from 1 / sqrt(hi);  abs: sign flip when hi < 0;  comparisons: lexicographic on (hi, lo)
@@ -116,6 +117,11 @@ DD_HD dd operator/(dd a, dd b) {
   return dd(q, e);
 }
 
+DD_HD dd& operator+=(dd& a, dd b) { return a = a + b; }
+DD_HD dd& operator-=(dd& a, dd b) { return a = a - b; }
+DD_HD dd& operator*=(dd& a, dd b) { return a = a * b; }
+DD_HD dd& operator/=(dd& a, dd b) { return a = a / b; }
+
 DD_HD bool operator==(dd a, dd b) { return a.hi == b.hi && a.lo == b.lo; }
 DD_HD bool operator!=(dd a, dd b) { return !(a == b); }
 DD_HD bool operator<(dd a, dd b) { return a.hi < b.hi || (a.hi == b.hi && a.lo < b.lo); }
@@ -163,6 +169,13 @@ DD_HD dd dd_abs_impl(dd re, dd im) {
   return sqrt(r * r + i * i) * small;
 }
 DD_HD dd dd_hypot(dd a, dd b) { return dd_abs_impl(a, b); }
+// overloads under the libm names, so that scalar templates (tridiag_dc_core.cuh) instantiate for dd
+using ::fmax;
+using ::fmin;
+using ::hypot;
+DD_HD dd fmax(dd a, dd b) { return a < b ? b : a; }
+DD_HD dd fmin(dd a, dd b) { return b < a ? b : a; }
+DD_HD dd hypot(dd a, dd b) { return dd_hypot(a, b); }
 
 #if defined(__CUDACC__)
 __device__ __forceinline__ dd __ldcg(const dd* p) {

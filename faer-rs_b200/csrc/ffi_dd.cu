@@ -241,6 +241,37 @@ void qr_recon_dd(FaerV0_24_MatMut A, FaerV0_24_MatRef Qb, FaerV0_24_MatRef Qc, F
   finish_all(st, {&a, &b, &f, &r});
 }
 
+// self-adjoint EVD (evd/mod.rs:270-418): the f64 / c64 entries' semantics (ffi.cu, ffi_types.cu); S holds (value, 0) for cx128
+template <bool CX>
+FaerV0_24_EvdStatus self_adjoint_evd_entry_dd(FaerV0_24_MatRef A, FaerV0_24_MatMut U, FaerV0_24_VecMut S) {
+  FB_ENTRY();
+  cudaStream_t st = current_stream();
+  const size_t n = A.nrows, e = es<CX>();
+  FB_ASSERT(A.ncols == n && S.len == n && (n == 0 || S.stride >= 1), "self_adjoint_evd: square A, S of length n, positive stride");
+  const bool want_u = U.ncols != 0;
+  if (want_u) FB_ASSERT(U.nrows == n && U.ncols == n, "self_adjoint_evd: U must be n x n (or have no columns)");
+  FaerV0_24_EvdStatus out;
+  memset(&out, 0, sizeof(out));
+  out.tag = FaerV0_24_EvdStatus_Ok;
+  if (n == 0) return out;
+  StagedMat a = stage<CX>(A, st);
+  dd* s_dev = (dd*)ws_alloc(n * e);
+  bool ok;
+  if (want_u) {
+    StagedMat u = stage<CX>(U, false, st);
+    ok = self_adjoint_evd_dd<CX>(st, a.view<const dd>(), u.view<dd>(), s_dev);
+    if (ok) FB_CUDA_CHECK(cudaMemcpy2DAsync(S.ptr, (size_t)S.stride * e, s_dev, e, e, n, cudaMemcpyDefault, st));
+    finish_all(st, {&a, &u});
+  } else {
+    ok = self_adjoint_evd_dd<CX>(st, a.view<const dd>(), View<dd>{nullptr, 0, 0, 1, 1}, s_dev);
+    if (ok) FB_CUDA_CHECK(cudaMemcpy2DAsync(S.ptr, (size_t)S.stride * e, s_dev, e, e, n, cudaMemcpyDefault, st));
+    finish_all(st, {&a});
+  }
+  ws_free(s_dev);
+  if (!ok) out.tag = FaerV0_24_EvdStatus_NoConvergence;
+  return out;
+}
+
 }  // namespace
 
 extern "C" {
@@ -504,5 +535,26 @@ FB_DD_LU_FFI(u64, 8, cx128, true)
 FB_DD_QR_FFI(fx128, false)
 FB_DD_QR_FFI(cx128, true)
 #undef FB_DD_QR_FFI
+
+// ---- self-adjoint EVD: faer's defaults (evd/mod.rs:82-90) and the f64 / c64 scratch formula with 16 / 32-byte elements ----
+#define FB_DD_EVD_FFI(SUF, CX)                                                                                                   \
+  FaerV0_24_TridiagParams libfaer_v0_23_TridiagParams_##SUF(void) { return FaerV0_24_TridiagParams{192 * 256}; }               \
+  FaerV0_24_SelfAdjointEvdParams libfaer_v0_23_SelfAdjointEvdParams_##SUF(void) {                                              \
+    return FaerV0_24_SelfAdjointEvdParams{FaerV0_24_TridiagParams{192 * 256}, 128};                                            \
+  }                                                                                                                            \
+  FaerV0_24_Layout libfaer_v0_23_self_adjoint_evd_scratch_##SUF(size_t dim, FaerV0_24_ComputeEigenvectors compute_U,           \
+                                                                FaerV0_24_Par par, FaerV0_24_SelfAdjointEvdParams params) {    \
+    (void)compute_U; (void)par; (void)params;                                                                                  \
+    return FaerV0_24_Layout{dim * dim * es<CX>(), 64};                                                                         \
+  }                                                                                                                            \
+  FaerV0_24_EvdStatus libfaer_v0_23_self_adjoint_evd_##SUF(FaerV0_24_MatRef A, FaerV0_24_MatMut U, FaerV0_24_VecMut S,         \
+                                                           FaerV0_24_Par par, FaerV0_24_MemAlloc mem,                          \
+                                                           FaerV0_24_SelfAdjointEvdParams params) {                            \
+    (void)par; (void)mem; (void)params;                                                                                        \
+    return self_adjoint_evd_entry_dd<CX>(A, U, S);                                                                             \
+  }
+FB_DD_EVD_FFI(fx128, false)
+FB_DD_EVD_FFI(cx128, true)
+#undef FB_DD_EVD_FFI
 
 }  // extern "C"

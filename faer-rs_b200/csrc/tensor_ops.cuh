@@ -27,6 +27,10 @@ template <bool CX>
 i64 qr_dd(cudaStream_t st, View<dd> A, View<dd> Q_coeff, i64 blocking_threshold);
 template <bool CX>
 void householder_sequence_dd(cudaStream_t st, View<const dd> basis, View<const dd> factor, bool conj, View<dd> rhs, bool transpose);
+// self-adjoint EVD (evd/mod.rs:270-418) of the matrix whose lower triangle is A; U with no columns: values only; S: n entries in
+// element units; false for non-finite input (evd_dd.cu)
+template <bool CX>
+bool self_adjoint_evd_dd(cudaStream_t st, View<const dd> A, View<dd> U, dd* S);
 
 inline void gemm(cudaStream_t st, VD dst, int ds, int accum, VCD lhs, int ls, VCD rhs, int rs, double alpha) {
   gemm_f64(st, dst, ds, accum, lhs, ls, rhs, rs, alpha);

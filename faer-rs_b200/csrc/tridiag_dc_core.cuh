@@ -12,6 +12,7 @@
 #pragma once
 #include <cfloat>
 #include <cmath>
+#include <type_traits>
 
 #ifdef __CUDACC__
 #define FB_HD __host__ __device__ __forceinline__
@@ -22,6 +23,23 @@
 namespace fb {
 namespace dc {
 
+// Unit roundoff-scale tolerance and underflow threshold of the scalar type. The double-double kind (fx128) specialises this, and
+// dc_sub below, in tridiag_dd.cuh; any other scalar type is rejected here.
+template <class T>
+struct DcLim {
+  static_assert(std::is_same<T, float>::value || std::is_same<T, double>::value,
+                "tridiag_dc_core.cuh: f32 / f64 only; the dd instantiation is in tridiag_dd.cuh");
+  static FB_HD T eps() { return sizeof(T) == 8 ? (T)DBL_EPSILON : (T)FLT_EPSILON; }
+  static FB_HD T tiny() { return sizeof(T) == 8 ? (T)DBL_MIN : (T)FLT_MIN; }
+};
+// a - b where the secular equation and the deflation need it to relative accuracy (differences of poles, and of a pole and a root).
+// An IEEE subtraction is exact to half an ulp of the result; dd specialises it with dd_sub_accurate, because dd's own subtraction
+// (faer's add(a, -b)) has an error of order 2^-106 |a| instead of 2^-106 |a - b|.
+template <class T>
+FB_HD T dc_sub(T a, T b) {
+  return a - b;
+}
+
 // ---- implicit QL with Wilkinson shifts on a small tridiagonal block (EISPACK tql2 recurrences) -------------------------
 // d[0..n): diagonal -> eigenvalues (unsorted); e[0..n): e[i] couples i and i+1 (e[n-1] unused / 0) -> destroyed.
 // The rotations are reported through `rot(i, c, s)`: columns i and i+1 of the eigenvector matrix are to be updated as
@@ -29,7 +47,7 @@ namespace dc {
 // Returns false if an eigenvalue needed more than 60 sweeps (does not happen for finite input).
 template <class T, class Rot>
 FB_HD bool ql_implicit(T* d, T* e, int n, Rot&& rot) {
-  const T eps = sizeof(T) == 8 ? (T)DBL_EPSILON : (T)FLT_EPSILON;
+  const T eps = DcLim<T>::eps();
   for (int l = 0; l < n; ++l) {
     int iter = 0;
     for (;;) {
@@ -85,7 +103,7 @@ FB_HD bool ql_implicit(T* d, T* e, int n, Rot&& rot) {
 template <class T>
 FB_HD int deflate_scan(T* d, T* z, const int* col, int s, T rho, T* dl, T* w, int* cnd, T* dd, int* cdf, int* rot_a, int* rot_b,
                        T* rot_c, T* rot_s, int* nrot_out) {
-  const T eps = sizeof(T) == 8 ? (T)DBL_EPSILON : (T)FLT_EPSILON;
+  const T eps = DcLim<T>::eps();
   T dmax = T(0), zmax = T(0);
   for (int i = 0; i < s; ++i) {
     dmax = fmax(dmax, fabs(d[i]));
@@ -114,7 +132,7 @@ FB_HD int deflate_scan(T* d, T* z, const int* col, int s, T rho, T* dl, T* w, in
     }
     T sn = z[pj], cs = z[j];
     const T tau = hypot(cs, sn);
-    const T t = d[j] - d[pj];
+    const T t = dc_sub(d[j], d[pj]);
     cs /= tau;
     sn = -sn / tau;
     if (fabs(t * cs * sn) <= tol) {
@@ -160,7 +178,7 @@ FB_HD T secular_f(const T* dl, const T* w, int k, int org, T tau, T rhoinv) {
   T f = rhoinv;
   const T dorg = dl[org];
   for (int i = 0; i < k; ++i) {
-    const T del = (dl[i] - dorg) - tau;
+    const T del = dc_sub(dc_sub(dl[i], dorg), tau);
     f += w[i] * (w[i] / del);
   }
   return f;
@@ -171,7 +189,7 @@ FB_HD T secular_root(const T* dl, int k, int j, T rho, T zz, Eval&& ev, int* org
   T lb, ub;
   int org;
   if (j < k - 1) {
-    const T half = (dl[j + 1] - dl[j]) * T(0.5);
+    const T half = dc_sub(dl[j + 1], dl[j]) * T(0.5);
     const T fmid = ev(j, half);
     if (fmid > T(0)) {  // root in the left half: origin dl[j], tau in (0, half]
       org = j;
@@ -191,7 +209,7 @@ FB_HD T secular_root(const T* dl, int k, int j, T rho, T zz, Eval&& ev, int* org
   }
   *org_out = org;
   // the open end of the bracket is a pole (tau = 0): move it inside, shrinking the ratio 2^-1, 2^-2, 2^-4, ...
-  const T tiny = sizeof(T) == 8 ? (T)DBL_MIN : (T)FLT_MIN;
+  const T tiny = DcLim<T>::tiny();
   if (lb == T(0)) {
     T t = T(0), fac = T(0.5);
     for (int it = 0; it < 12; ++it) {
