@@ -7,16 +7,12 @@
 //     d = Re(a_jj); [regularise]; fail with Err(j) if !(d > 0); l_jj = sqrt(d); fail if l_jj == 0 or non-finite;
 //     column j (INCLUDING the diagonal entry) is multiplied by recip(l_jj).
 //
-// GPU mapping: recursive blocked driver on the host stream; the <=128-wide diagonal block is factored by ONE CTA:
-//   * 16 "update" warps hold the block in REGISTERS (thread (lane, w) owns rows lane+32a, columns w+16b) and apply the
-//     reference's per-element FMA chain (same k order, same reciprocal-multiply, diagonal scaled too) => bit-identical
-//     to the reference leaf recurrence;
-//   * 4 "pivot" warps keep a redundant copy of the diagonal (updated with the very same FMA sequence, so bit-identical)
-//     and do the serial pivot arithmetic (regularise, test, sqrt, reciprocal) of column j+1 WHILE the update warps are
-//     still applying column j — the sqrt+divide latency is off the update warps' critical path;
-//   * each column costs one __syncthreads; the unscaled pivot column travels through a double-buffered shared vector.
+// GPU mapping: recursive blocked driver on the host stream; the <=128-wide diagonal block is factored by ONE CTA that
+// keeps it in shared memory and works through it in 32-column panels without a CTA barrier per column (potf2_kernel).
 // The panel solve is G3 and the trailing update is the lower-masked DMMA GEMM (G2). A device status word carries the
 // first failing column / the regularisation count and is read back once per factorisation.
+#include <atomic>
+
 #include "gemm_f32.cuh"
 #include "linalg_f64.cuh"
 
@@ -25,12 +21,18 @@ namespace fb {
 namespace {
 
 constexpr int POTF2_MAX = 128;
-constexpr int POTF2_UPD_WARPS = 16;
-constexpr int POTF2_THREADS = POTF2_UPD_WARPS * 32 + POTF2_MAX;  // 512 update threads + 128 pivot threads
-constexpr int POTF2_CB = POTF2_MAX / POTF2_UPD_WARPS;           // column slots per update thread (8)
+constexpr int POTF2_W = 32;                             // panel width: one diagonal-block row per lane
+constexpr int POTF2_PANEL_WARPS = POTF2_MAX / POTF2_W;  // warps that factor a panel, 32 rows each
+constexpr int POTF2_WARPS = 8;
+constexpr int POTF2_THREADS = POTF2_WARPS * 32;
+constexpr int POTF2_TN = 4;                             // trailing update: columns per warp tile
 
 __device__ __forceinline__ double recip_rn(double x) { return __drcp_rn(x); }
 __device__ __forceinline__ float recip_rn(float x) { return __frcp_rn(x); }
+template <class T>
+struct __align__(2 * sizeof(T)) Pair {
+  T x, y;
+};
 
 // scalar-type dispatch of the two building blocks the recursion calls (G3 solve, lower-masked GEMM)
 inline void solve_lower(cudaStream_t st, VCD tri, bool unit, VD rhs) { solve_lower_triangular_in_place_f64(st, tri, unit, rhs); }
@@ -39,133 +41,181 @@ inline void solve_lower(cudaStream_t st, VCF tri, bool unit, VF rhs) { solve_low
 inline void gemm_lower_update(cudaStream_t st, VD dst, VCD a) { gemm_f64(st, dst, TRI_LOWER, 1, a, RECT, a.t(), RECT, -1.0); }
 inline void gemm_lower_update(cudaStream_t st, VF dst, VCF a) { gemm_f32(st, dst, TRI_LOWER, 1, a, RECT, a.t(), RECT, -1.0f); }
 
-// info[0]: first failing global column (or -1), info[1]: regularisation count
+// One CTA factors an n <= 128 diagonal block held in shared memory, S[c * POTF2_MAX + i] = a_ic, in 32-column panels:
+//   1. warps 0-3 factor the panel: warp w holds the panel's rows p0 + 32w + lane in registers (warp 0: the diagonal
+//      block's rows), and every one of them also holds the diagonal block's rows and factors that block itself, warp
+//      synchronously: the pivot comes from lane c by shuffle, the column of L travels through a warp-private buffer.
+//      Warps 1-3 thereby run the forward substitution of the rows below the diagonal block without waiting for warp 0;
+//   2. all warps apply the panel to the trailing lower triangle (32 FMAs per element).
+// Three CTA barriers per panel instead of one per column. The arithmetic is the reference leaf's, element by element:
+// a_ic <- fma(-l_ck, l_ik, a_ic) for k = 0..c-1 in ascending order, l_xk = (updated a_xk) * recip_rn(sqrt(d_k)), and
+// the diagonal entry is scaled with the rest of its column; the four warps compute the diagonal block's bits
+// identically, so the pivot decisions are the same in all of them and every branch below is warp- or CTA-uniform.
+// info[0]: first failing global column (or -1), info[1]: regularisation count. On a failure at column f, columns < f
+// hold L and the rest of A is left as it was; the count is not added.
 template <class T>
-__global__ void __launch_bounds__(POTF2_THREADS) potf2_kernel(T* __restrict__ A, i64 rs, i64 cs, int n, i64 j0,
-                                                               int regularize, T eps, T delta,
-                                                               long long* __restrict__ info) {
-  __shared__ T colbuf[2][POTF2_MAX];
-  __shared__ T s_inv[2];
-  __shared__ int s_fail[2];
-  __shared__ int s_count;
+__global__ void __launch_bounds__(POTF2_THREADS, 1) potf2_kernel(T* __restrict__ A, i64 rs, i64 cs, int n, i64 j0,
+                                                                  int regularize, T eps, T delta,
+                                                                  long long* __restrict__ info) {
+  extern __shared__ __align__(16) unsigned char potf2_smem[];
+  T* S = reinterpret_cast<T*>(potf2_smem);  // columns 0 .. roundup(n, 32) - 1
+  __shared__ __align__(16) T colv[POTF2_PANEL_WARPS][2][2 * POTF2_W];
+  __shared__ int s_fail, s_count;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const bool is_upd = warp < POTF2_UPD_WARPS;
-  const int p = tid - POTF2_UPD_WARPS * 32;  // pivot-thread index (diagonal entry p) when !is_upd
   if (info[0] >= 0) return;  // an earlier block already failed (uniform across the CTA)
-  if (tid == 0) s_count = 0;
 
-  // update threads: rows i = lane + 32a, columns c = warp + 16b, kept iff c <= i < n
-  T a[4][POTF2_CB];
-  T dp = T(0);  // pivot threads: diagonal entry p
-  if (is_upd) {
-#pragma unroll
-    for (int ai = 0; ai < 4; ++ai)
-#pragma unroll
-      for (int bi = 0; bi < POTF2_CB; ++bi) {
-        const int i = lane + 32 * ai, c = warp + POTF2_UPD_WARPS * bi;
-        a[ai][bi] = (i < n && c <= i) ? A[(i64)i * rs + (i64)c * cs] : T(0);
-      }
-  } else if (p < n) {
-    dp = A[(i64)p * rs + (i64)p * cs];
+  // the whole block in flight at once, zero-filled outside the lower triangle
+  const int ncol = (n + POTF2_W - 1) & ~(POTF2_W - 1);
+  for (int e = tid; e < ncol * POTF2_MAX; e += POTF2_THREADS) {
+    const int i = e % POTF2_MAX, c = e / POTF2_MAX;
+    const bool ok = i < n && c <= i;
+    const T* src = ok ? A + (i64)i * rs + (i64)c * cs : A;
+    if constexpr (sizeof(T) == 8) cp_async_8(S + e, src, ok ? 8 : 0);
+    else cp_async_4(S + e, src, ok ? 4 : 0);
   }
-  __syncthreads();  // s_count initialised
-
-  // serial pivot arithmetic of column jc (reference ldlt/factor.rs:122-160), done by ONE pivot thread
-  auto publish_pivot = [&](int jc, T d) {
-    int fail = 0;
-    if (regularize) {
-      if (d <= eps) {  // LLT: sign == +1
-        d = delta;
-        s_count += 1;  // single writer per column, ordered by the per-column barrier
-      }
-    }
-    T inv = T(0);
-    if (!(d > T(0))) {
-      fail = 1;
-    } else {
-      const T sd = sqrt(d);
-      if (sd == T(0) || !isfinite(sd)) fail = 1;
-      else inv = recip_rn(sd);  // correctly rounded reciprocal = T(1) / sd bit for bit, without the division's slow path
-    }
-    s_inv[jc & 1] = inv;
-    s_fail[jc & 1] = fail;
-  };
-
-  if (is_upd) {
-    if (warp == 0) {
-#pragma unroll
-      for (int ai = 0; ai < 4; ++ai) colbuf[0][lane + 32 * ai] = a[ai][0];
-    }
-  } else if (p == 0) {
-    publish_pivot(0, dp);
+  cp_async_commit();
+  cp_async_wait<0>();
+  if (tid == 0) {
+    s_fail = -1;
+    s_count = 0;
   }
   __syncthreads();
 
-  for (int j = 0; j < n; ++j) {
-    const T* col = colbuf[j & 1];
-    if (s_fail[j & 1]) {
-      if (tid == 0) info[0] = j0 + j;
-      return;
+  for (int p0 = 0; p0 < n; p0 += POTF2_W) {
+    T* P = S + p0 * POTF2_MAX;  // the panel's first column
+    const int wp = min(POTF2_W, n - p0);
+    const int r = p0 + POTF2_W * warp + lane;  // this lane's row of the panel
+    const bool factors = warp < POTF2_PANEL_WARPS && p0 + POTF2_W * warp < n;
+    T ad[POTF2_W], ar[POTF2_W];  // row p0 + lane of the diagonal block, row r of the panel
+    if (factors) {
+#pragma unroll
+      for (int c = 0; c < POTF2_W; ++c) {
+        ad[c] = P[c * POTF2_MAX + p0 + lane];
+        ar[c] = P[c * POTF2_MAX + r];
+      }
     }
-    const T inv = s_inv[j & 1];
-    if (!is_upd) {
-      // pivot group: keep the diagonal current with the SAME fma the update threads apply to a_pp, then start the
-      // next column's pivot arithmetic immediately
-      if (p > j && p < n) {
-        const T l = col[p] * inv;
-        dp = fma(-l, l, dp);
-        if (p == j + 1) publish_pivot(j + 1, dp);
-      }
-    } else {
-      const int jw = j & (POTF2_UPD_WARPS - 1);
-      // column j of L goes to global memory (owners: warp jw).
-      // NB: like the reference, the stored diagonal is (unregularised a_jj) * recip(l_jj)
-      // (ldlt/factor.rs:161-175 scales the whole column, diagonal included, and `diag` is a local copy).
-      if (warp == jw) {
-#pragma unroll
-        for (int ai = 0; ai < 4; ++ai) {
-          const int i = lane + 32 * ai;
-          if (i >= j && i < n) A[(i64)i * rs + (i64)j * cs] = col[i] * inv;
+    __syncthreads();  // every copy of the diagonal block is read before warp 0 overwrites it with L
+
+    if (factors) {
+      int cnt = 0, fail = -1;
+      T dn = ad[0];  // lane c: the diagonal entry of column c, updated through column c - 1
+      // One rolled iteration per column, so that the loop stays in the instruction cache: fully unrolled over the 32
+      // columns the kernel was ~8k instructions, and inside the LLT step, where the bulk update keeps L2 busy, its
+      // instruction fetches made it 3x slower than on an idle GPU. ad[k] / ar[k] hold column c + k, and each column's
+      // update also shifts the rows down by one slot (ad[k] <- fma(., ., ad[k + 1])), so the current column is always
+      // slot 0 and every register index stays a compile-time constant.
+#pragma unroll 1
+      for (int c = 0; c < wp; ++c) {
+        // pivot (reference ldlt/factor.rs:122-160); d is the same in every lane
+        T d = __shfl_sync(0xffffffffu, dn, c);
+        if (regularize) {
+          if (d <= eps) {  // LLT: sign == +1
+            d = delta;
+            ++cnt;
+          }
         }
-      }
-      // trailing update: a_ic <- fma(-l_cj, l_ij, a_ic) for j < c <= i. The column test depends only on
-      // (warp, bi, j): warp-uniform, so dead column slots are BRANCHED over (no predicated-off instruction issue).
-      if (warp + POTF2_UPD_WARPS * (POTF2_CB - 1) > j) {
-        T li[4];
+        T inv = T(0);
+        bool bad = !(d > T(0));
+        if (!bad) {
+          const T sd = sqrt(d);
+          if (sd == T(0) || !isfinite(sd)) bad = true;
+          else inv = recip_rn(sd);  // correctly rounded reciprocal = T(1) / sd bit for bit, without the division's slow path
+        }
+        if (bad) {
+          fail = p0 + c;
+          break;
+        }
+        // NB: like the reference, the stored diagonal is (unregularised a_cc) * recip(l_cc)
+        // (ldlt/factor.rs:161-175 scales the whole column, diagonal included, and `diag` is a local copy).
+        const T ld = ad[0] * inv, lr = ar[0] * inv;
+        if (r >= p0 + c && r < n) P[c * POTF2_MAX + r] = lr;
+        // l of diagonal-block row `lane` goes to slot W - 1 + lane - c: the entry of column c + 1 + k is slot W + k
+        T* cv = colv[warp][c & 1];  // double-buffered: column c + 1 writes the other half
+        cv[POTF2_W - 1 + lane - c] = ld;
+        __syncwarp();
+        dn = fma(-ld, ld, ad[1]);  // lane c + 1's own l: the next pivot does not wait for the buffer
+        const int live = wp - 1 - c;  // columns of the panel after c; slots from `live` on are never read again
+        const Pair<T>* cp = reinterpret_cast<const Pair<T>*>(cv + POTF2_W);
 #pragma unroll
-        for (int ai = 0; ai < 4; ++ai) li[ai] = col[lane + 32 * ai] * inv;
-#pragma unroll
-        for (int bi = 0; bi < POTF2_CB; ++bi) {
-          const int c = warp + POTF2_UPD_WARPS * bi;
-          if (c > j && c < n) {
-            const T lc = col[c] * inv;
-#pragma unroll
-            for (int ai = 0; ai < 4; ++ai) {
-              const int i = lane + 32 * ai;
-              if (32 * ai + 31 >= c) {  // warp-uniform: this row slot intersects i >= c
-                if (i >= c && i < n) a[ai][bi] = fma(-lc, li[ai], a[ai][bi]);
-              }
-            }
+        for (int q = 0; q < POTF2_W / 2; ++q) {
+          if (q % 4 == 0 && 2 * q >= live) break;  // warp-uniform, in steps of 8 slots
+          const Pair<T> l2 = cp[q];
+          ad[2 * q] = fma(-l2.x, ld, ad[2 * q + 1]);
+          ar[2 * q] = fma(-l2.x, lr, ar[2 * q + 1]);
+          if (2 * q + 2 < POTF2_W) {
+            ad[2 * q + 1] = fma(-l2.y, ld, ad[2 * q + 2]);
+            ar[2 * q + 1] = fma(-l2.y, lr, ar[2 * q + 2]);
           }
         }
       }
-      // owners of column j+1 publish it (unscaled) into the other buffer
-      if (j + 1 < n && warp == ((j + 1) & (POTF2_UPD_WARPS - 1))) {
-        const int nbk = (j + 1) / POTF2_UPD_WARPS;
-        T* nxt = colbuf[(j + 1) & 1];
-#pragma unroll
-        for (int ai = 0; ai < 4; ++ai) {
-          T v = T(0);
-#pragma unroll
-          for (int bi = 0; bi < POTF2_CB; ++bi)
-            if (bi == nbk) v = a[ai][bi];
-          nxt[lane + 32 * ai] = v;
-        }
+      if (tid == 0) {
+        s_count += cnt;
+        s_fail = fail;
       }
     }
     __syncthreads();
+    if (s_fail >= 0) break;
+
+    // trailing update of columns [p0 + 32, n): warp tiles of 4 columns x 128 rows, row slots below the diagonal only
+    for (int cg = p0 + POTF2_W + POTF2_TN * warp; cg < n; cg += POTF2_TN * POTF2_WARPS) {
+      T acc[4][POTF2_TN];
+#pragma unroll
+      for (int a = 0; a < 4; ++a)
+#pragma unroll
+        for (int j = 0; j < POTF2_TN; ++j) acc[a][j] = S[(cg + j) * POTF2_MAX + 32 * a + lane];
+#pragma unroll
+      for (int k = 0; k < POTF2_W; ++k) {
+        const T* Lk = P + k * POTF2_MAX;
+        T lc[POTF2_TN];
+#pragma unroll
+        for (int j = 0; j < POTF2_TN; ++j) lc[j] = Lk[cg + j];
+#pragma unroll
+        for (int a = 0; a < 4; ++a) {
+          if (32 * a + 31 >= cg && 32 * a < n) {  // warp-uniform: the slot meets the lower triangle
+            const T li = Lk[32 * a + lane];
+#pragma unroll
+            for (int j = 0; j < POTF2_TN; ++j) acc[a][j] = fma(-lc[j], li, acc[a][j]);
+          }
+        }
+      }
+#pragma unroll
+      for (int a = 0; a < 4; ++a)
+        if (32 * a + 31 >= cg && 32 * a < n)
+#pragma unroll
+          for (int j = 0; j < POTF2_TN; ++j) S[(cg + j) * POTF2_MAX + 32 * a + lane] = acc[a][j];
+    }
+    __syncthreads();
   }
-  if (tid == 0 && s_count) info[1] += s_count;
+
+  const int fail = s_fail;
+  const int done = fail >= 0 ? fail : n;  // columns of L to store
+  for (int e = tid; e < done * POTF2_MAX; e += POTF2_THREADS) {
+    const int i = e % POTF2_MAX, c = e / POTF2_MAX;
+    if (i >= c && i < n) A[(i64)i * rs + (i64)c * cs] = S[e];
+  }
+  if (tid == 0) {
+    if (fail >= 0) info[0] = j0 + fail;
+    else if (s_count) info[1] += s_count;
+  }
+}
+
+// potf2_kernel on the block; the shared-memory opt-in is set once per device
+template <class T>
+void potf2(cudaStream_t stream, View<T> A, i64 j0, int regularize, T eps, T delta, long long* d_info) {
+  static std::atomic<unsigned long long> opted{0};
+  int dev = 0;
+  FB_CUDA_CHECK(cudaGetDevice(&dev));
+  FB_ASSERT(dev < 64, "device index out of range");
+  if (!(opted.load() >> dev & 1)) {
+    FB_CUDA_CHECK(cudaFuncSetAttribute(potf2_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       (int)(POTF2_MAX * POTF2_MAX * sizeof(T))));
+    opted.fetch_or(1ull << dev);
+  }
+  const int n = (int)A.nrows;
+  const size_t smem = (size_t)((n + POTF2_W - 1) / POTF2_W * POTF2_W) * POTF2_MAX * sizeof(T);
+  potf2_kernel<T><<<1, POTF2_THREADS, smem, stream>>>(A.ptr, A.rs, A.cs, n, j0, regularize, eps, delta, d_info);
+  FB_CUDA_CHECK(cudaGetLastError());
+  note_launch();
 }
 
 template <class T>
@@ -185,10 +235,7 @@ template <class T>
 void llt_rec(const LltCtx<T>& ctx, View<T> A, i64 j0) {
   const i64 n = A.nrows;
   if (n <= ctx.nb) {
-    potf2_kernel<T><<<1, POTF2_THREADS, 0, ctx.stream>>>(A.ptr, A.rs, A.cs, (int)n, j0, ctx.regularize, ctx.eps, ctx.delta,
-                                                      ctx.d_info);
-    FB_CUDA_CHECK(cudaGetLastError());
-    note_launch();
+    potf2<T>(ctx.stream, A, j0, ctx.regularize, ctx.eps, ctx.delta, ctx.d_info);
     return;
   }
   // split at a multiple of the leaf size closest to n/2
