@@ -561,12 +561,11 @@ FaerV0_24_ColPivQrStatus colpiv_qr_factor_entry(FaerV0_24_MatMut A, FaerV0_24_Ma
   FB_ASSERT(size == 0 || Q_coeff.nrows > 0, "Q_coeff.nrows (the block size) must be positive (the reference would not terminate)");
   FB_ASSERT(A.ncols == 0 || (perm_fwd.ptr != nullptr && perm_bwd.ptr != nullptr), "null permutation slice");
   cudaStream_t st = current_stream();
-  const size_t es = (CX ? 2 : 1) * sizeof(R);
   std::vector<long long> trans, fwd, bwd;
   i64 count = 0;
   if (size > 0) {
-    StagedMat a(A.ptr, (i64)A.nrows, (i64)A.ncols, (i64)A.row_stride, (i64)A.col_stride, es, true, true, st);
-    StagedMat q(Q_coeff.ptr, (i64)Q_coeff.nrows, (i64)Q_coeff.ncols, (i64)Q_coeff.row_stride, (i64)Q_coeff.col_stride, es, true, true, st);
+    StagedMat a = stage<R, CX>(A, true, st);
+    StagedMat q = stage<R, CX>(Q_coeff, true, st);
     count = colpiv_qr_in_place_t<R, CX>(st, a.view<R>(), q.view<R>(), A.row_stride == 1, trans);
     finish_all(st, {&a, &q});
   }
@@ -586,8 +585,7 @@ FaerV0_24_ColPivQrStatus colpiv_qr_factor_entry(FaerV0_24_MatMut A, FaerV0_24_Ma
 template <class R, bool CX, class F>
 void cpq_staged(FaerV0_24_MatMut M, size_t nrows, const std::vector<long long>& perm, bool cols, bool perm_first, F&& unpivoted) {
   cudaStream_t st = current_stream();
-  const size_t es = (CX ? 2 : 1) * sizeof(R);
-  StagedMat s(M.ptr, (i64)M.nrows, (i64)M.ncols, (i64)M.row_stride, (i64)M.col_stride, es, true, true, st);
+  StagedMat s = stage<R, CX>(M, true, st);
   View<R> v = s.view<R>();
   const FaerV0_24_MatMut dm{(void*)v.ptr, M.nrows, M.ncols, (ptrdiff_t)v.rs, (ptrdiff_t)v.cs};
   View<R> pv = cols ? View<R>{v.ptr, v.ncols, v.nrows, v.cs, v.rs} : v;

@@ -1,6 +1,6 @@
-// Helpers shared by the translation units of the extern "C" boundary (ffi.cu, ffi_types.cu and the pivoted factorizations): scalar /
-// permutation arguments that may live on the host or on the device, the end-of-call sequence of the staged matrices, and the
-// permutations and scratch layouts the pivoted families return.
+// Helpers shared by the translation units of the extern "C" boundary (ffi.cu, ffi_types.cu, ffi_dd.cu and the pivoted
+// factorizations): staging of matrix arguments, scalar / permutation arguments that may live on the host or on the device, the
+// end-of-call sequence of the staged matrices, the statuses, and the permutations and scratch layouts the pivoted families return.
 #pragma once
 #include "../../include/faer_b200.h"
 #include "runtime.cuh"
@@ -14,17 +14,30 @@
 namespace fb {
 // (static, not an anonymous namespace: nvcc's kernel stubs of a unit that also has a global anonymous namespace must stay unambiguous)
 
-static inline double read_scalar_f64(const FaerV0_24_Scalar* p) {
-  FB_ASSERT(p != nullptr, "null scalar pointer");
-  double v;
-  if (is_device_pointer(p)) {
-    FB_CUDA_CHECK(cudaMemcpy(&v, p, sizeof(double), cudaMemcpyDeviceToHost));
-  } else {
-    memcpy(&v, p, sizeof(double));
-  }
-  return v;
+// bytes of one element of the scalar kind <R, complex?>
+template <class R, bool CX>
+static constexpr size_t elem_bytes() {
+  return (CX ? 2 : 1) * sizeof(R);
 }
 
+// A matrix argument of the kind <R, CX> as a device view: inputs are copied in and never back, outputs are copied back (and in
+// only with `copy_in`)
+template <class R, bool CX>
+static StagedMat stage(FaerV0_24_MatRef m, cudaStream_t st) {
+  return StagedMat(m.ptr, (i64)m.nrows, (i64)m.ncols, (i64)m.row_stride, (i64)m.col_stride, elem_bytes<R, CX>(), true, false, st);
+}
+template <class R, bool CX>
+static StagedMat stage(FaerV0_24_MatMut m, bool copy_in, cudaStream_t st) {
+  return StagedMat(m.ptr, (i64)m.nrows, (i64)m.ncols, (i64)m.row_stride, (i64)m.col_stride, elem_bytes<R, CX>(), copy_in, true, st);
+}
+
+// one scalar of the kind <R, CX> (`CX ? 2 : 1` values of R) from a host or device pointer; real parameters (T::Real) are <R, false>
+template <class R, bool CX = false>
+static void read_scalar(const void* p, R* out) {
+  FB_ASSERT(p != nullptr, "null scalar pointer");
+  if (is_device_pointer(p)) FB_CUDA_CHECK(cudaMemcpy(out, p, elem_bytes<R, CX>(), cudaMemcpyDeviceToHost));
+  else memcpy((void*)out, p, elem_bytes<R, CX>());
+}
 
 static inline void finish_all(cudaStream_t st, std::initializer_list<StagedMat*> mats) {
   // the compute must be complete before input mirrors return to the pool; calls are synchronous anyway
@@ -32,14 +45,61 @@ static inline void finish_all(cudaStream_t st, std::initializer_list<StagedMat*>
   for (auto* m : mats) m->finish();
 }
 
-
-static inline double read_real(const void* p, double) { return read_scalar_f64((const FaerV0_24_Scalar*)p); }
-static inline float read_real(const void* p, float) {
-  FB_ASSERT(p != nullptr, "null scalar pointer");
-  float v;
-  if (is_device_pointer(p)) FB_CUDA_CHECK(cudaMemcpy(&v, p, sizeof(float), cudaMemcpyDeviceToHost));
-  else memcpy(&v, p, sizeof(float));
-  return v;
+// the statuses of the entry points, from the drivers' results
+static inline FaerV0_24_LltStatus llt_status(const LltResult& r) {
+  FaerV0_24_LltStatus out;
+  memset(&out, 0, sizeof(out));
+  if (r.ok) {
+    out.tag = FaerV0_24_LltStatus_Ok;
+    out.ok.dynamic_regularization_count = r.dynamic_regularization_count;
+  } else {
+    out.tag = FaerV0_24_LltStatus_NonPositivePivot;
+    out.non_positive_pivot.index = r.non_positive_pivot_index;
+  }
+  return out;
+}
+static inline FaerV0_24_LdltStatus ldlt_status(const LdltResult& r) {
+  FaerV0_24_LdltStatus out;
+  memset(&out, 0, sizeof(out));
+  if (r.ok) {
+    out.tag = FaerV0_24_LdltStatus_Ok;
+    out.ok.dynamic_regularization_count = r.dynamic_regularization_count;
+  } else {
+    out.tag = FaerV0_24_LdltStatus_ZeroPivot;
+    out.zero_pivot.index = r.zero_pivot_index;
+  }
+  return out;
+}
+static inline FaerV0_24_PartialPivLuStatus partial_piv_lu_status(size_t transposition_count) {
+  FaerV0_24_PartialPivLuStatus out;
+  memset(&out, 0, sizeof(out));
+  out.tag = FaerV0_24_PartialPivLuStatus_Ok;
+  out.ok.transposition_count = transposition_count;
+  return out;
+}
+// `negative_is_unknown`: a negative rank means QrStatus::Unknown; otherwise the rank is taken as it is
+static inline FaerV0_24_QrStatus qr_status(i64 rank, bool negative_is_unknown) {
+  FaerV0_24_QrStatus out;
+  memset(&out, 0, sizeof(out));
+  if (negative_is_unknown && rank < 0) {
+    out.tag = FaerV0_24_QrStatus_Unknown;
+  } else {
+    out.tag = FaerV0_24_QrStatus_Ok;
+    out.ok.rank = (size_t)rank;
+  }
+  return out;
+}
+static inline FaerV0_24_EvdStatus evd_status(bool ok) {
+  FaerV0_24_EvdStatus out;
+  memset(&out, 0, sizeof(out));
+  out.tag = ok ? FaerV0_24_EvdStatus_Ok : FaerV0_24_EvdStatus_NoConvergence;
+  return out;
+}
+static inline FaerV0_24_SvdStatus svd_status(bool ok) {
+  FaerV0_24_SvdStatus out;
+  memset(&out, 0, sizeof(out));
+  out.tag = ok ? FaerV0_24_SvdStatus_Ok : FaerV0_24_SvdStatus_NoConvergence;
+  return out;
 }
 
 // index slices (u32 / u64) <-> host int64

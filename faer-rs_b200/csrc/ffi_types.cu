@@ -1,62 +1,18 @@
 // extern "C" boundary, second translation unit: the entry points whose drivers are the flat-map files (reconstruct_types.cu,
-// ldlt_types.cu, cplx_condensed.cu) — `*_reconstruct` / `*_inverse` for f32 / c64 / c32, LDLT beyond the f64 factorization, `svd` /
-// `self_adjoint_evd` for complex T. Same conventions as ffi.cu (by-value PODs, synchronous on return, abort() on precondition
+// ldlt_types.cu, cplx_condensed.cu) — `*_reconstruct` / `*_inverse` for f32 / c64 / c32 and the triangular inverses (both
+// instantiated from ffi_entries.cuh), LDLT beyond the f64 factorization, `svd` / `self_adjoint_evd` for complex T. Same conventions as ffi.cu (by-value PODs, synchronous on return, abort() on precondition
 // violations, host buffers staged, device buffers used in place). Kept apart from ffi.cu so that this unit, runtime.cu and the
 // three drivers also build for the host (tools/emul/ffi_types_host.cpp: the staging layer and the drivers end to end on the CPU).
 #include "ffi_common.cuh"
+#include "ffi_entries.cuh"
 #include "flat_map.cuh"
 #include "gemm_f32.cuh"
 #include "runtime.cuh"
 #include "tensor_ops.cuh"
 
-#include <memory>
-
 using namespace fb;
 
 namespace {
-
-// ---- reconstruct / inverse on the factors for f32 / c64 / c32 (reconstruct_types.cu; scalar kind <R, CX>) ----
-template <class R, bool CX>
-void llt_recon_entry_t(FaerV0_24_MatMut A, FaerV0_24_MatRef L, bool inverse) {
-  FB_ENTRY();
-  cudaStream_t st = current_stream();
-  const size_t es = (CX ? 2 : 1) * sizeof(R);
-  // only the lower triangle is written: the rest of A must survive the round trip
-  StagedMat a(A.ptr, (i64)A.nrows, (i64)A.ncols, (i64)A.row_stride, (i64)A.col_stride, es, true, true, st);
-  StagedMat l(L.ptr, (i64)L.nrows, (i64)L.ncols, (i64)L.row_stride, (i64)L.col_stride, es, true, false, st);
-  if (inverse) llt_inverse_t<R, CX>(st, a.view<R>(), l.view<const R>());
-  else llt_reconstruct_t<R, CX>(st, a.view<R>(), l.view<const R>());
-  finish_all(st, {&a, &l});
-}
-template <class R, bool CX>
-void lu_recon_entry_t(FaerV0_24_MatMut A, FaerV0_24_MatRef L, FaerV0_24_MatRef U, FaerV0_24_SliceRef perm, int idx_bytes,
-                      bool inverse) {
-  FB_ENTRY();
-  cudaStream_t st = current_stream();
-  const size_t es = (CX ? 2 : 1) * sizeof(R);
-  const size_t m = L.nrows;
-  std::vector<long long> p = read_perm(perm.ptr, m, idx_bytes);
-  for (size_t i = 0; i < m; ++i) FB_ASSERT(p[i] >= 0 && (size_t)p[i] < m, "invalid permutation entry");
-  StagedMat a(A.ptr, (i64)A.nrows, (i64)A.ncols, (i64)A.row_stride, (i64)A.col_stride, es, false, true, st);
-  StagedMat l(L.ptr, (i64)L.nrows, (i64)L.ncols, (i64)L.row_stride, (i64)L.col_stride, es, true, false, st);
-  StagedMat u(U.ptr, (i64)U.nrows, (i64)U.ncols, (i64)U.row_stride, (i64)U.col_stride, es, true, false, st);
-  if (inverse) lu_inverse_t<R, CX>(st, a.view<R>(), l.view<const R>(), u.view<const R>(), p.data());
-  else lu_reconstruct_t<R, CX>(st, a.view<R>(), l.view<const R>(), u.view<const R>(), p.data());
-  finish_all(st, {&a, &l, &u});
-}
-template <class R, bool CX>
-void qr_recon_entry_t(FaerV0_24_MatMut A, FaerV0_24_MatRef Q_basis, FaerV0_24_MatRef Q_coeff, FaerV0_24_MatRef Rm, bool inverse) {
-  FB_ENTRY();
-  cudaStream_t st = current_stream();
-  const size_t es = (CX ? 2 : 1) * sizeof(R);
-  StagedMat a(A.ptr, (i64)A.nrows, (i64)A.ncols, (i64)A.row_stride, (i64)A.col_stride, es, false, true, st);
-  StagedMat b(Q_basis.ptr, (i64)Q_basis.nrows, (i64)Q_basis.ncols, (i64)Q_basis.row_stride, (i64)Q_basis.col_stride, es, true, false, st);
-  StagedMat f(Q_coeff.ptr, (i64)Q_coeff.nrows, (i64)Q_coeff.ncols, (i64)Q_coeff.row_stride, (i64)Q_coeff.col_stride, es, true, false, st);
-  StagedMat r(Rm.ptr, (i64)Rm.nrows, (i64)Rm.ncols, (i64)Rm.row_stride, (i64)Rm.col_stride, es, true, false, st);
-  if (inverse) qr_inverse_t<R, CX>(st, a.view<R>(), b.view<const R>(), f.view<const R>(), r.view<const R>());
-  else qr_reconstruct_t<R, CX>(st, a.view<R>(), b.view<const R>(), f.view<const R>(), r.view<const R>());
-  finish_all(st, {&a, &b, &f, &r});
-}
 
 // ---- `svd` / `self_adjoint_evd` for complex T (cplx_condensed.cu); S holds T-typed entries (value, 0), strides in complex units ----
 template <class R>
@@ -67,15 +23,12 @@ FaerV0_24_EvdStatus self_adjoint_evd_entry_cplx(FaerV0_24_MatRef A, FaerV0_24_Ma
   FB_ASSERT(A.ncols == n && S.len == n && (n == 0 || S.stride >= 1), "self_adjoint_evd: square A, S of length n, positive stride");
   const bool want_u = U.ncols != 0;
   if (want_u) FB_ASSERT(U.nrows == n && U.ncols == n, "self_adjoint_evd: U must be n x n (or have no columns)");
-  FaerV0_24_EvdStatus out;
-  memset(&out, 0, sizeof(out));
-  out.tag = FaerV0_24_EvdStatus_Ok;
-  if (n == 0) return out;
-  StagedMat a(A.ptr, (i64)n, (i64)n, (i64)A.row_stride, (i64)A.col_stride, es, true, false, st);
+  if (n == 0) return evd_status(true);
+  StagedMat a = stage<R, true>(A, st);
   R* s_dev = (R*)ws_alloc(n * es);
   bool ok;
   if (want_u) {
-    StagedMat u(U.ptr, (i64)n, (i64)n, (i64)U.row_stride, (i64)U.col_stride, es, false, true, st);
+    StagedMat u = stage<R, true>(U, false, st);
     ok = self_adjoint_evd_cx<R>(st, a.view<const R>(), u.view<R>(), s_dev, 1);
     if (ok) FB_CUDA_CHECK(cudaMemcpy2DAsync(S.ptr, (size_t)S.stride * es, s_dev, es, es, n, cudaMemcpyDefault, st));
     finish_all(st, {&a, &u});
@@ -85,8 +38,7 @@ FaerV0_24_EvdStatus self_adjoint_evd_entry_cplx(FaerV0_24_MatRef A, FaerV0_24_Ma
     finish_all(st, {&a});
   }
   ws_free(s_dev);
-  if (!ok) out.tag = FaerV0_24_EvdStatus_NoConvergence;
-  return out;
+  return evd_status(ok);
 }
 template <class R>
 FaerV0_24_SvdStatus svd_entry_cplx(FaerV0_24_MatRef A, FaerV0_24_MatMut U, FaerV0_24_VecMut S, FaerV0_24_MatMut V) {
@@ -97,16 +49,12 @@ FaerV0_24_SvdStatus svd_entry_cplx(FaerV0_24_MatRef A, FaerV0_24_MatMut U, FaerV
   const bool want_u = U.ncols != 0, want_v = V.ncols != 0;
   if (want_u) FB_ASSERT(U.nrows == A.nrows && (U.ncols == A.nrows || U.ncols == size), "svd: U must be nrows x {size, nrows}");
   if (want_v) FB_ASSERT(V.nrows == A.ncols && (V.ncols == A.ncols || V.ncols == size), "svd: V must be ncols x {size, ncols}");
-  FaerV0_24_SvdStatus out;
-  memset(&out, 0, sizeof(out));
-  out.tag = FaerV0_24_SvdStatus_Ok;
-  if (size == 0 && !want_u && !want_v) return out;
-  StagedMat a(A.ptr, (i64)A.nrows, (i64)A.ncols, (i64)A.row_stride, (i64)A.col_stride, es, true, false, st);
+  if (size == 0 && !want_u && !want_v) return svd_status(true);
+  StagedMat a = stage<R, true>(A, st);
   R* s_dev = (R*)ws_alloc((size + 1) * es);
   bool ok;
   if (want_u || want_v) {
-    StagedMat u(U.ptr, (i64)U.nrows, (i64)U.ncols, (i64)U.row_stride, (i64)U.col_stride, es, false, true, st);
-    StagedMat v(V.ptr, (i64)V.nrows, (i64)V.ncols, (i64)V.row_stride, (i64)V.col_stride, es, false, true, st);
+    StagedMat u = stage<R, true>(U, false, st), v = stage<R, true>(V, false, st);
     View<R> uv = want_u ? u.view<R>() : View<R>{nullptr, 0, 0, 1, 1};
     View<R> vv = want_v ? v.view<R>() : View<R>{nullptr, 0, 0, 1, 1};
     ok = svd_cx<R>(st, a.view<const R>(), uv, s_dev, 1, vv);
@@ -118,8 +66,7 @@ FaerV0_24_SvdStatus svd_entry_cplx(FaerV0_24_MatRef A, FaerV0_24_MatMut U, FaerV
     finish_all(st, {&a});
   }
   ws_free(s_dev);
-  if (!ok) out.tag = FaerV0_24_SvdStatus_NoConvergence;
-  return out;
+  return svd_status(ok);
 }
 
 // ---- LDLT for the other scalar kinds (ldlt_types.cu); D arrives as a VecRef of T-typed entries ----
@@ -153,10 +100,9 @@ FaerV0_24_LdltStatus ldlt_factor_entry_t(FaerV0_24_MatMut A, FaerV0_24_LdltRegul
   FB_ENTRY();
   FB_ASSERT(A.nrows == A.ncols, "LDLT needs a square matrix");
   cudaStream_t st = current_stream();
-  const size_t es = (CX ? 2 : 1) * sizeof(R);
   R delta = 0, eps = 0;  // the regularisation parameters are T::Real
-  if (regularization.dynamic_regularization_delta) delta = read_real(regularization.dynamic_regularization_delta, R());
-  if (regularization.dynamic_regularization_epsilon) eps = read_real(regularization.dynamic_regularization_epsilon, R());
+  if (regularization.dynamic_regularization_delta) read_scalar<R>(regularization.dynamic_regularization_delta, &delta);
+  if (regularization.dynamic_regularization_epsilon) read_scalar<R>(regularization.dynamic_regularization_epsilon, &eps);
   const signed char* d_signs = nullptr;
   signed char* signs_mirror = nullptr;
   const FaerV0_24_SliceMut sg = regularization.dynamic_regularization_signs;
@@ -170,30 +116,20 @@ FaerV0_24_LdltStatus ldlt_factor_entry_t(FaerV0_24_MatMut A, FaerV0_24_LdltRegul
       d_signs = signs_mirror;
     }
   }
-  StagedMat a(A.ptr, (i64)A.nrows, (i64)A.ncols, (i64)A.row_stride, (i64)A.col_stride, es, true, true, st);
+  StagedMat a = stage<R, CX>(A, true, st);
   const LdltResult r = ldlt_in_place_t<R, CX>(st, a.view<R>(), delta, eps, d_signs);
   finish_all(st, {&a});
   if (signs_mirror) ws_free(signs_mirror);
-  FaerV0_24_LdltStatus out;
-  memset(&out, 0, sizeof(out));
-  if (r.ok) {
-    out.tag = FaerV0_24_LdltStatus_Ok;
-    out.ok.dynamic_regularization_count = r.dynamic_regularization_count;
-  } else {
-    out.tag = FaerV0_24_LdltStatus_ZeroPivot;
-    out.zero_pivot.index = r.zero_pivot_index;
-  }
-  return out;
+  return ldlt_status(r);
 }
 template <class R, bool CX>
 void ldlt_solve_entry_t(FaerV0_24_MatRef L, FaerV0_24_VecRef D, FaerV0_24_Conj A_conj, FaerV0_24_MatMut rhs) {
   FB_ENTRY();
   cudaStream_t st = current_stream();
-  const size_t n = L.nrows, es = (CX ? 2 : 1) * sizeof(R);
+  const size_t n = L.nrows;
   FB_ASSERT(L.ncols == n && D.len == n && rhs.nrows == n, "LDLT solve shape mismatch");
   if (n == 0 || rhs.ncols == 0) return;
-  StagedMat l(L.ptr, (i64)n, (i64)n, (i64)L.row_stride, (i64)L.col_stride, es, true, false, st);
-  StagedMat r(rhs.ptr, (i64)rhs.nrows, (i64)rhs.ncols, (i64)rhs.row_stride, (i64)rhs.col_stride, es, true, true, st);
+  StagedMat l = stage<R, CX>(L, st), r = stage<R, CX>(rhs, true, st);
   DiagArg<R, CX> d(D, n, st);
   ldlt_solve_in_place_t<R, CX>(st, l.view<const R>(), d.ptr, d.stride, A_conj == FaerV0_24_Conj_Yes, r.view<R>());
   finish_all(st, {&l, &r});
@@ -202,12 +138,11 @@ template <class R, bool CX>
 void ldlt_recon_entry_t(FaerV0_24_MatMut A, FaerV0_24_MatRef L, FaerV0_24_VecRef D, bool inverse) {
   FB_ENTRY();
   cudaStream_t st = current_stream();
-  const size_t n = L.nrows, es = (CX ? 2 : 1) * sizeof(R);
+  const size_t n = L.nrows;
   FB_ASSERT(L.ncols == n && D.len == n && A.nrows == n && A.ncols == n, "LDLT reconstruct / inverse shape mismatch");
   if (n == 0) return;
   // only the lower triangle is written: the rest of A must survive the round trip
-  StagedMat a(A.ptr, (i64)n, (i64)n, (i64)A.row_stride, (i64)A.col_stride, es, true, true, st);
-  StagedMat l(L.ptr, (i64)n, (i64)n, (i64)L.row_stride, (i64)L.col_stride, es, true, false, st);
+  StagedMat a = stage<R, CX>(A, true, st), l = stage<R, CX>(L, st);
   DiagArg<R, CX> d(D, n, st);
   if (inverse) ldlt_inverse_t<R, CX>(st, a.view<R>(), l.view<const R>(), d.ptr, d.stride);
   else ldlt_reconstruct_t<R, CX>(st, a.view<R>(), l.view<const R>(), d.ptr, d.stride);
@@ -255,9 +190,7 @@ template <class T>
 void bidiag_entry(FaerV0_24_MatMut A, FaerV0_24_MatMut Hl, FaerV0_24_MatMut Hr) {
   FB_ENTRY();
   cudaStream_t st = current_stream();
-  StagedMat a(A.ptr, (i64)A.nrows, (i64)A.ncols, (i64)A.row_stride, (i64)A.col_stride, sizeof(T), true, true, st);
-  StagedMat hl(Hl.ptr, (i64)Hl.nrows, (i64)Hl.ncols, (i64)Hl.row_stride, (i64)Hl.col_stride, sizeof(T), true, true, st);
-  StagedMat hr(Hr.ptr, (i64)Hr.nrows, (i64)Hr.ncols, (i64)Hr.row_stride, (i64)Hr.col_stride, sizeof(T), true, true, st);
+  StagedMat a = stage<T, false>(A, true, st), hl = stage<T, false>(Hl, true, st), hr = stage<T, false>(Hr, true, st);
   ColMajorWork<T> w(st, a.view<T>());
   bidiag_in_place<T>(st, w.work, hl.view<T>(), hr.view<T>());
   w.finish();
@@ -267,27 +200,11 @@ template <class T>
 void tridiag_entry(FaerV0_24_MatMut A, FaerV0_24_MatMut H) {
   FB_ENTRY();
   cudaStream_t st = current_stream();
-  StagedMat a(A.ptr, (i64)A.nrows, (i64)A.ncols, (i64)A.row_stride, (i64)A.col_stride, sizeof(T), true, true, st);
-  StagedMat h(H.ptr, (i64)H.nrows, (i64)H.ncols, (i64)H.row_stride, (i64)H.col_stride, sizeof(T), true, true, st);
+  StagedMat a = stage<T, false>(A, true, st), h = stage<T, false>(H, true, st);
   ColMajorWork<T> w(st, a.view<T>());
   tridiag_in_place<T>(st, w.work, h.view<T>());
   w.finish();
   finish_all(st, {&a, &h});
-}
-
-// ---- triangular inverses (triangular_inverse.rs; faer-ffi/src/lib.rs:938-980) ----
-template <class R, bool CX>
-void inverse_triangular_entry_t(FaerV0_24_MatMut dst, FaerV0_24_MatRef src, bool lower, bool unit) {
-  FB_ENTRY();
-  cudaStream_t st = current_stream();
-  const size_t es = (CX ? 2 : 1) * sizeof(R);
-  FB_ASSERT(dst.nrows == dst.ncols && src.nrows == dst.nrows && src.ncols == dst.ncols, "inverse_triangular shape mismatch");
-  if (dst.nrows == 0) return;
-  // only the triangle is written: the rest of dst must survive the round trip
-  StagedMat d(dst.ptr, (i64)dst.nrows, (i64)dst.ncols, (i64)dst.row_stride, (i64)dst.col_stride, es, true, true, st);
-  StagedMat s(src.ptr, (i64)src.nrows, (i64)src.ncols, (i64)src.row_stride, (i64)src.col_stride, es, true, false, st);
-  inverse_triangular_t<R, CX>(st, d.view<R>(), s.view<const R>(), lower, unit);
-  finish_all(st, {&d, &s});
 }
 
 // ---- Hessenberg reduction (extension; evd/hessenberg.rs:549-567) ----
@@ -295,10 +212,8 @@ template <class R, bool CX>
 void hessenberg_entry_t(FaerV0_24_MatMut A, FaerV0_24_MatMut H) {
   FB_ENTRY();
   cudaStream_t st = current_stream();
-  const size_t es = (CX ? 2 : 1) * sizeof(R);
   FB_ASSERT(A.nrows == A.ncols && H.ncols == (A.nrows > 0 ? A.nrows - 1 : 0), "hessenberg_in_place: square A, householder factor bs x (n - 1)");
-  StagedMat a(A.ptr, (i64)A.nrows, (i64)A.ncols, (i64)A.row_stride, (i64)A.col_stride, es, true, true, st);
-  StagedMat h(H.ptr, (i64)H.nrows, (i64)H.ncols, (i64)H.row_stride, (i64)H.col_stride, es, false, true, st);
+  StagedMat a = stage<R, CX>(A, true, st), h = stage<R, CX>(H, false, st);
   hessenberg_in_place_t<R, CX>(st, a.view<R>(), h.view<R>());
   finish_all(st, {&a, &h});
 }
@@ -308,10 +223,7 @@ template <class R>
 void bidiag_entry_cx(FaerV0_24_MatMut A, FaerV0_24_MatMut Hl, FaerV0_24_MatMut Hr) {
   FB_ENTRY();
   cudaStream_t st = current_stream();
-  const size_t es = 2 * sizeof(R);
-  StagedMat a(A.ptr, (i64)A.nrows, (i64)A.ncols, (i64)A.row_stride, (i64)A.col_stride, es, true, true, st);
-  StagedMat hl(Hl.ptr, (i64)Hl.nrows, (i64)Hl.ncols, (i64)Hl.row_stride, (i64)Hl.col_stride, es, false, true, st);
-  StagedMat hr(Hr.ptr, (i64)Hr.nrows, (i64)Hr.ncols, (i64)Hr.row_stride, (i64)Hr.col_stride, es, false, true, st);
+  StagedMat a = stage<R, true>(A, true, st), hl = stage<R, true>(Hl, false, st), hr = stage<R, true>(Hr, false, st);
   bidiag_in_place_cx<R>(st, a.view<R>(), hl.view<R>(), hr.view<R>());
   finish_all(st, {&a, &hl, &hr});
 }
@@ -319,9 +231,7 @@ template <class R>
 void tridiag_entry_cx(FaerV0_24_MatMut A, FaerV0_24_MatMut H) {
   FB_ENTRY();
   cudaStream_t st = current_stream();
-  const size_t es = 2 * sizeof(R);
-  StagedMat a(A.ptr, (i64)A.nrows, (i64)A.ncols, (i64)A.row_stride, (i64)A.col_stride, es, true, true, st);
-  StagedMat h(H.ptr, (i64)H.nrows, (i64)H.ncols, (i64)H.row_stride, (i64)H.col_stride, es, false, true, st);
+  StagedMat a = stage<R, true>(A, true, st), h = stage<R, true>(H, false, st);
   tridiag_in_place_cx<R>(st, a.view<R>(), h.view<R>());
   finish_all(st, {&a, &h});
 }
@@ -381,78 +291,23 @@ FB_SVD_EVD_CPLX_FFI(c64, double)
 FB_SVD_EVD_CPLX_FFI(c32, float)
 #undef FB_SVD_EVD_CPLX_FFI
 
-// ---- reconstruct / inverse for f32 / c64 / c32 (scratch sizes: the f64 formulas above with the element size of T) ----
-#define FB_RECON_TYPES_FFI(SUF, R, CX, ES)                                                                                       \
-  FaerV0_24_Layout libfaer_v0_23_llt_reconstruct_scratch_##SUF(size_t dim, FaerV0_24_Par par) {                                 \
-    (void)dim; (void)par;                                                                                                       \
-    return FaerV0_24_Layout{0, 1};                                                                                              \
-  }                                                                                                                             \
-  void libfaer_v0_23_llt_reconstruct_##SUF(FaerV0_24_MatMut A, FaerV0_24_MatRef L, FaerV0_24_Par par, FaerV0_24_MemAlloc mem) { \
-    (void)par; (void)mem;                                                                                                       \
-    llt_recon_entry_t<R, CX>(A, L, false);                                                                                      \
-  }                                                                                                                             \
-  FaerV0_24_Layout libfaer_v0_23_llt_inverse_scratch_##SUF(size_t dim, FaerV0_24_Par par) {                                     \
-    (void)par;                                                                                                                  \
-    return FaerV0_24_Layout{dim * dim * (ES), 64};                                                                              \
-  }                                                                                                                             \
-  void libfaer_v0_23_llt_inverse_##SUF(FaerV0_24_MatMut A_inv, FaerV0_24_MatRef L, FaerV0_24_Par par, FaerV0_24_MemAlloc mem) { \
-    (void)par; (void)mem;                                                                                                       \
-    llt_recon_entry_t<R, CX>(A_inv, L, true);                                                                                   \
-  }                                                                                                                             \
-  FaerV0_24_Layout libfaer_v0_23_qr_inverse_scratch_##SUF(size_t dim, size_t block_size, FaerV0_24_Par par) {                   \
-    (void)par;                                                                                                                  \
-    return FaerV0_24_Layout{block_size * dim * (ES), 64};                                                                       \
-  }                                                                                                                             \
-  void libfaer_v0_23_qr_inverse_##SUF(FaerV0_24_MatMut A, FaerV0_24_MatRef Q_basis, FaerV0_24_MatRef Q_coeff, FaerV0_24_MatRef R_, \
-                                      FaerV0_24_Par par, FaerV0_24_MemAlloc mem) {                                              \
-    (void)par; (void)mem;                                                                                                       \
-    qr_recon_entry_t<R, CX>(A, Q_basis, Q_coeff, R_, true);                                                                     \
-  }
-#define FB_QR_RECON_TYPES_FFI(SUF, R, CX, ES)                                                                                    \
-  FaerV0_24_Layout libfaer_v0_23_qr_reconstruct_scratch_##SUF(size_t nrows, size_t ncols, size_t block_size, FaerV0_24_Par par) { \
-    (void)nrows; (void)par;                                                                                                     \
-    return FaerV0_24_Layout{block_size * ncols * (ES), 64};                                                                     \
-  }                                                                                                                             \
-  void libfaer_v0_23_qr_reconstruct_##SUF(FaerV0_24_MatMut A, FaerV0_24_MatRef Q_basis, FaerV0_24_MatRef Q_coeff,               \
-                                          FaerV0_24_MatRef R_, FaerV0_24_Par par, FaerV0_24_MemAlloc mem) {                     \
-    (void)par; (void)mem;                                                                                                       \
-    qr_recon_entry_t<R, CX>(A, Q_basis, Q_coeff, R_, false);                                                                    \
-  }
-#define FB_LU_RECON_TYPES_FFI(IT, BYTES, SUF, R, CX, ES)                                                                         \
-  FaerV0_24_Layout libfaer_v0_23_partial_piv_lu_reconstruct_scratch_##IT##_##SUF(size_t nrows, size_t ncols, FaerV0_24_Par par) { \
-    (void)par;                                                                                                                  \
-    return FaerV0_24_Layout{nrows * ncols * (ES), 64};                                                                          \
-  }                                                                                                                             \
-  void libfaer_v0_23_partial_piv_lu_reconstruct_##IT##_##SUF(FaerV0_24_MatMut A, FaerV0_24_MatRef L, FaerV0_24_MatRef U,        \
-                                                             FaerV0_24_SliceRef perm_fwd, FaerV0_24_SliceRef perm_bwd,          \
-                                                             FaerV0_24_Par par, FaerV0_24_MemAlloc mem) {                       \
-    (void)perm_fwd; (void)par; (void)mem;                                                                                       \
-    lu_recon_entry_t<R, CX>(A, L, U, perm_bwd, BYTES, false);                                                                   \
-  }                                                                                                                             \
-  FaerV0_24_Layout libfaer_v0_23_partial_piv_lu_inverse_scratch_##IT##_##SUF(size_t dim, FaerV0_24_Par par) {                   \
-    (void)par;                                                                                                                  \
-    return FaerV0_24_Layout{dim * dim * (ES), 64};                                                                              \
-  }                                                                                                                             \
-  void libfaer_v0_23_partial_piv_lu_inverse_##IT##_##SUF(FaerV0_24_MatMut A, FaerV0_24_MatRef L, FaerV0_24_MatRef U,            \
-                                                         FaerV0_24_SliceRef perm_fwd, FaerV0_24_SliceRef perm_bwd,              \
-                                                         FaerV0_24_Par par, FaerV0_24_MemAlloc mem) {                           \
-    (void)perm_bwd; (void)par; (void)mem;                                                                                       \
-    lu_recon_entry_t<R, CX>(A, L, U, perm_fwd, BYTES, true);                                                                    \
-  }
-FB_RECON_TYPES_FFI(f32, float, false, sizeof(float))
-FB_RECON_TYPES_FFI(c64, double, true, 2 * sizeof(double))
-FB_RECON_TYPES_FFI(c32, float, true, 2 * sizeof(float))
-FB_QR_RECON_TYPES_FFI(c64, double, true, 2 * sizeof(double))
-FB_QR_RECON_TYPES_FFI(c32, float, true, 2 * sizeof(float))
-FB_LU_RECON_TYPES_FFI(u32, 4, f32, float, false, sizeof(float))
-FB_LU_RECON_TYPES_FFI(u64, 8, f32, float, false, sizeof(float))
-FB_LU_RECON_TYPES_FFI(u32, 4, c64, double, true, 2 * sizeof(double))
-FB_LU_RECON_TYPES_FFI(u64, 8, c64, double, true, 2 * sizeof(double))
-FB_LU_RECON_TYPES_FFI(u32, 4, c32, float, true, 2 * sizeof(float))
-FB_LU_RECON_TYPES_FFI(u64, 8, c32, float, true, 2 * sizeof(float))
-#undef FB_RECON_TYPES_FFI
-#undef FB_QR_RECON_TYPES_FFI
-#undef FB_LU_RECON_TYPES_FFI
+// ---- reconstruct / inverse for f32 / c64 / c32 (ffi_entries.cuh; qr_reconstruct_f32 is in ffi.cu) and the triangular inverses of
+// every IEEE kind ----
+FB_LLT_RECON_FFI(f32, float, false)
+FB_LLT_RECON_FFI(c64, double, true)
+FB_LLT_RECON_FFI(c32, float, true)
+FB_LU_RECON_FFI(f32, float, false)
+FB_LU_RECON_FFI(c64, double, true)
+FB_LU_RECON_FFI(c32, float, true)
+FB_QR_RECON_FFI(c64, double, true)
+FB_QR_RECON_FFI(c32, float, true)
+FB_QR_INV_FFI(f32, float, false)
+FB_QR_INV_FFI(c64, double, true)
+FB_QR_INV_FFI(c32, float, true)
+FB_TRI_INV_FFI(f64, double, false)
+FB_TRI_INV_FFI(f32, float, false)
+FB_TRI_INV_FFI(c64, double, true)
+FB_TRI_INV_FFI(c32, float, true)
 
 // ---- LDLT: factor / solve for f32 / c64 / c32, reconstruct / inverse for every dtype (ldlt_types.cu) ----
 #define FB_LDLT_FS_FFI(SUF, R, CX, ES)                                                                                          \
@@ -504,30 +359,6 @@ FB_LDLT_RI_FFI(c64, double, true, 2 * sizeof(double))
 FB_LDLT_RI_FFI(c32, float, true, 2 * sizeof(float))
 #undef FB_LDLT_FS_FFI
 #undef FB_LDLT_RI_FFI
-
-// ---- triangular inverses, every dtype ----
-#define FB_TRI_INV_FFI(SUF, R, CX)                                                                                              \
-  void libfaer_v0_23_inverse_triangular_lower_in_place_##SUF(FaerV0_24_MatMut L_inv, FaerV0_24_MatRef L, FaerV0_24_Par par) {    \
-    (void)par;                                                                                                                  \
-    inverse_triangular_entry_t<R, CX>(L_inv, L, true, false);                                                                   \
-  }                                                                                                                             \
-  void libfaer_v0_23_inverse_triangular_upper_in_place_##SUF(FaerV0_24_MatMut L_inv, FaerV0_24_MatRef L, FaerV0_24_Par par) {    \
-    (void)par;                                                                                                                  \
-    inverse_triangular_entry_t<R, CX>(L_inv, L, false, false);                                                                  \
-  }                                                                                                                             \
-  void libfaer_v0_23_inverse_unit_triangular_lower_in_place_##SUF(FaerV0_24_MatMut L_inv, FaerV0_24_MatRef L, FaerV0_24_Par par) { \
-    (void)par;                                                                                                                  \
-    inverse_triangular_entry_t<R, CX>(L_inv, L, true, true);                                                                    \
-  }                                                                                                                             \
-  void libfaer_v0_23_inverse_unit_triangular_upper_in_place_##SUF(FaerV0_24_MatMut L_inv, FaerV0_24_MatRef L, FaerV0_24_Par par) { \
-    (void)par;                                                                                                                  \
-    inverse_triangular_entry_t<R, CX>(L_inv, L, false, true);                                                                   \
-  }
-FB_TRI_INV_FFI(f64, double, false)
-FB_TRI_INV_FFI(f32, float, false)
-FB_TRI_INV_FFI(c64, double, true)
-FB_TRI_INV_FFI(c32, float, true)
-#undef FB_TRI_INV_FFI
 
 FaerV0_24_HessenbergParams libfaer_v0_23_HessenbergParams_f64(void) { return FaerV0_24_HessenbergParams{192 * 256, 256 * 256}; }
 FaerV0_24_HessenbergParams libfaer_v0_23_HessenbergParams_f32(void) { return FaerV0_24_HessenbergParams{192 * 256, 256 * 256}; }

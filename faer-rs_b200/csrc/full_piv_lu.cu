@@ -408,13 +408,12 @@ FaerV0_24_FullPivLuStatus full_piv_lu_factor_entry(FaerV0_24_MatMut A, FaerV0_24
   FB_ASSERT(m == 0 || (row_fwd.ptr != nullptr && row_bwd.ptr != nullptr), "null row permutation slice");
   FB_ASSERT(n == 0 || (col_fwd.ptr != nullptr && col_bwd.ptr != nullptr), "null column permutation slice");
   cudaStream_t st = current_stream();
-  const size_t es = (CX ? 2 : 1) * sizeof(R);
   std::vector<long long> rt, ct;
   i64 count = 0;
   if (m > 0 && n > 0) {
     // the branch reads the CALLER's strides (factor.rs:492): the staged mirror may be laid out differently
     const bool transpose = !(std::llabs((long long)A.row_stride) < std::llabs((long long)A.col_stride));
-    StagedMat a(A.ptr, (i64)m, (i64)n, (i64)A.row_stride, (i64)A.col_stride, es, true, true, st);
+    StagedMat a = stage<R, CX>(A, true, st);
     count = full_piv_lu_in_place_t<R, CX>(st, a.view<R>(), transpose, rt, ct);
     finish_all(st, {&a});
   }
@@ -441,12 +440,11 @@ void full_piv_lu_solve_entry(FaerV0_24_MatRef L, FaerV0_24_MatRef U, FaerV0_24_C
   const size_t n = L.nrows;
   FB_ASSERT(L.ncols == n && U.nrows == n && U.ncols == n && rhs.nrows == n, "full-pivoting LU solve shape mismatch");
   cudaStream_t st = current_stream();
-  const size_t es = (CX ? 2 : 1) * sizeof(R);
   const std::vector<long long> rf = read_perm_checked(row_fwd, n, idx_bytes), rb = read_perm_checked(row_bwd, n, idx_bytes);
   const std::vector<long long> cf = read_perm_checked(col_fwd, n, idx_bytes), cb = read_perm_checked(col_bwd, n, idx_bytes);
-  StagedMat l(L.ptr, (i64)n, (i64)n, (i64)L.row_stride, (i64)L.col_stride, es, true, false, st);
-  StagedMat u(U.ptr, (i64)n, (i64)n, (i64)U.row_stride, (i64)U.col_stride, es, true, false, st);
-  StagedMat r(rhs.ptr, (i64)rhs.nrows, (i64)rhs.ncols, (i64)rhs.row_stride, (i64)rhs.col_stride, es, true, true, st);
+  StagedMat l = stage<R, CX>(L, st);
+  StagedMat u = stage<R, CX>(U, st);
+  StagedMat r = stage<R, CX>(rhs, true, st);
   full_piv_lu_solve_t<R, CX>(st, l.view<const R>(), u.view<const R>(), rf.data(), rb.data(), cf.data(), cb.data(),
                              conj == FaerV0_24_Conj_Yes, transpose, r.view<R>());
   finish_all(st, {&l, &u, &r});
@@ -463,11 +461,10 @@ void full_piv_lu_recon_entry(FaerV0_24_MatMut A, FaerV0_24_MatRef L, FaerV0_24_M
     FB_ASSERT(A.nrows == m && A.ncols == n && L.ncols >= (m < n ? m : n) && U.nrows >= (m < n ? m : n),
               "full-pivoting LU reconstruct shape mismatch");
   cudaStream_t st = current_stream();
-  const size_t es = (CX ? 2 : 1) * sizeof(R);
   const std::vector<long long> rb = read_perm_checked(row_bwd, m, idx_bytes), cb = read_perm_checked(col_bwd, n, idx_bytes);
-  StagedMat a(A.ptr, (i64)A.nrows, (i64)A.ncols, (i64)A.row_stride, (i64)A.col_stride, es, false, true, st);
-  StagedMat l(L.ptr, (i64)L.nrows, (i64)L.ncols, (i64)L.row_stride, (i64)L.col_stride, es, true, false, st);
-  StagedMat u(U.ptr, (i64)U.nrows, (i64)U.ncols, (i64)U.row_stride, (i64)U.col_stride, es, true, false, st);
+  StagedMat a = stage<R, CX>(A, false, st);
+  StagedMat l = stage<R, CX>(L, st);
+  StagedMat u = stage<R, CX>(U, st);
   if (inverse) full_piv_lu_inverse_t<R, CX>(st, a.view<R>(), l.view<const R>(), u.view<const R>(), rb.data(), cb.data());
   else full_piv_lu_reconstruct_t<R, CX>(st, a.view<R>(), l.view<const R>(), u.view<const R>(), rb.data(), cb.data());
   finish_all(st, {&a, &l, &u});

@@ -1108,7 +1108,7 @@ FaerV0_24_LbltStatus lblt_factor_entry(FaerV0_24_MatMut A, FaerV0_24_VecMut subd
   FB_ASSERT(subdiag.ptr != nullptr && (subdiag.stride >= 1 || n == 1), "LBLT subdiag needs a positive stride");
   cudaStream_t st = current_stream();
   const size_t es = (CX ? 2 : 1) * sizeof(R);
-  StagedMat a(A.ptr, (i64)n, (i64)n, (i64)A.row_stride, (i64)A.col_stride, es, true, true, st);
+  StagedMat a = stage<R, CX>(A, true, st);
   const i64 sstride = n == 1 ? 1 : (i64)subdiag.stride;
   StagedMat s(subdiag.ptr, (i64)n, 1, sstride, (i64)n * sstride, es, true, true, st);
   std::vector<unsigned long long> piv;
@@ -1140,8 +1140,8 @@ void lblt_solve_entry(FaerV0_24_MatRef L, FaerV0_24_VecRef diag, FaerV0_24_VecRe
   const size_t es = (CX ? 2 : 1) * sizeof(R);
   const std::vector<long long> pf = read_perm_checked(perm_fwd, n, idx_bytes), pb = read_perm_checked(perm_bwd, n, idx_bytes);
   const std::vector<unsigned char> dg = lb_read_vec(diag.ptr, n, diag.stride, es), sd = lb_read_vec(subdiag.ptr, n, subdiag.stride, es);
-  StagedMat l(L.ptr, (i64)n, (i64)n, (i64)L.row_stride, (i64)L.col_stride, es, true, false, st);
-  StagedMat r(rhs.ptr, (i64)rhs.nrows, (i64)rhs.ncols, (i64)rhs.row_stride, (i64)rhs.col_stride, es, true, true, st);
+  StagedMat l = stage<R, CX>(L, st);
+  StagedMat r = stage<R, CX>(rhs, true, st);
   lblt_solve_t<R, CX>(st, l.view<const R>(), dg, sd, pf.data(), pb.data(), A_conj == FaerV0_24_Conj_Yes, r.view<R>());
   finish_all(st, {&l, &r});
 }
@@ -1160,8 +1160,8 @@ void lblt_recon_entry(FaerV0_24_MatMut A, FaerV0_24_MatRef L, FaerV0_24_VecRef d
   const std::vector<long long> pf = read_perm_checked(perm_fwd, n, idx_bytes), pb = read_perm_checked(perm_bwd, n, idx_bytes);
   const std::vector<unsigned char> sd = lb_read_vec(subdiag.ptr, n, subdiag.stride, es);
   // every entry of the output is written
-  StagedMat a(A.ptr, (i64)n, (i64)n, (i64)A.row_stride, (i64)A.col_stride, es, false, true, st);
-  StagedMat l(L.ptr, (i64)n, (i64)n, (i64)L.row_stride, (i64)L.col_stride, es, true, false, st);
+  StagedMat a = stage<R, CX>(A, false, st);
+  StagedMat l = stage<R, CX>(L, st);
   if (inverse) {
     const std::vector<unsigned char> dg = lb_read_vec(diag.ptr, n, diag.stride, es);
     lblt_inverse_t<R, CX>(st, a.view<R>(), l.view<const R>(), dg, sd, pf.data(), pb.data());

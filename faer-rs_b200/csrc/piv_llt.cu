@@ -591,8 +591,7 @@ FaerV0_24_PivLltStatus piv_llt_factor_entry(FaerV0_24_MatMut A, FaerV0_24_SliceM
   // the permutation length is A.nrows, never SliceMut.len (see lu_entry in ffi.cu)
   FB_ASSERT(A.nrows == 0 || (perm_fwd.ptr != nullptr && perm_bwd.ptr != nullptr), "null permutation slice");
   cudaStream_t st = current_stream();
-  const size_t es = (CX ? 2 : 1) * sizeof(R);
-  StagedMat a(A.ptr, (i64)A.nrows, (i64)A.ncols, (i64)A.row_stride, (i64)A.col_stride, es, true, true, st);
+  StagedMat a = stage<R, CX>(A, true, st);
   std::vector<long long> trans, fwd, bwd;
   const PivLltResult r = piv_llt_in_place_t<R, CX>(st, a.view<R>(), (i64)params.block_size, trans);
   finish_all(st, {&a});
@@ -618,10 +617,10 @@ void piv_llt_solve_entry(FaerV0_24_MatRef L, FaerV0_24_SliceRef perm_fwd, FaerV0
   FB_ENTRY();
   FB_ASSERT(L.nrows == L.ncols && rhs.nrows == L.nrows, "pivoted LLT solve shape mismatch");
   cudaStream_t st = current_stream();
-  const size_t es = (CX ? 2 : 1) * sizeof(R), n = L.nrows;
+  const size_t n = L.nrows;
   std::vector<long long> pf = read_perm_checked(perm_fwd, n, idx_bytes), pb = read_perm_checked(perm_bwd, n, idx_bytes);
-  StagedMat l(L.ptr, (i64)L.nrows, (i64)L.ncols, (i64)L.row_stride, (i64)L.col_stride, es, true, false, st);
-  StagedMat r(rhs.ptr, (i64)rhs.nrows, (i64)rhs.ncols, (i64)rhs.row_stride, (i64)rhs.col_stride, es, true, true, st);
+  StagedMat l = stage<R, CX>(L, st);
+  StagedMat r = stage<R, CX>(rhs, true, st);
   piv_llt_solve_t<R, CX>(st, l.view<const R>(), pf.data(), pb.data(), A_conj == FaerV0_24_Conj_Yes, r.view<R>());
   finish_all(st, {&l, &r});
 }
@@ -631,11 +630,11 @@ void piv_llt_recon_entry(FaerV0_24_MatMut A, FaerV0_24_MatRef L, FaerV0_24_Slice
   FB_ENTRY();
   FB_ASSERT(L.nrows == L.ncols && A.nrows == L.nrows && A.ncols == L.nrows, "pivoted LLT reconstruct / inverse shape mismatch");
   cudaStream_t st = current_stream();
-  const size_t es = (CX ? 2 : 1) * sizeof(R), n = L.nrows;
+  const size_t n = L.nrows;
   std::vector<long long> pb = read_perm_checked(perm_bwd, n, idx_bytes);
   // only the lower triangle is written: the rest of A must survive the round trip
-  StagedMat a(A.ptr, (i64)A.nrows, (i64)A.ncols, (i64)A.row_stride, (i64)A.col_stride, es, true, true, st);
-  StagedMat l(L.ptr, (i64)L.nrows, (i64)L.ncols, (i64)L.row_stride, (i64)L.col_stride, es, true, false, st);
+  StagedMat a = stage<R, CX>(A, true, st);
+  StagedMat l = stage<R, CX>(L, st);
   piv_llt_recon_t<R, CX>(st, a.view<R>(), l.view<const R>(), pb.data(), inverse);
   finish_all(st, {&a, &l});
 }

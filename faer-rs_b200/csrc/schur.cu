@@ -424,13 +424,10 @@ FaerV0_24_EvdStatus evd_entry(FaerV0_24_MatRef A, FaerV0_24_MatMut UL, FaerV0_24
   const bool want_l = UL.ncols != 0, want_r = UR.ncols != 0;
   if (want_l) FB_ASSERT(UL.nrows == n && UL.ncols == n, "evd: UL must be n x n (or have no columns)");
   if (want_r) FB_ASSERT(UR.nrows == n && UR.ncols == n, "evd: UR must be n x n (or have no columns)");
-  FaerV0_24_EvdStatus out;
-  memset(&out, 0, sizeof(out));
-  out.tag = FaerV0_24_EvdStatus_Ok;
-  if (n == 0) return out;
+  if (n == 0) return evd_status(true);
   size_t ns_limit = ~(size_t)0;
   if (params.schur.recommended_shift_count) ns_limit = params.schur.recommended_shift_count(n, n);
-  StagedMat a(A.ptr, (i64)n, (i64)n, (i64)A.row_stride, (i64)A.col_stride, es, true, false, st);
+  StagedMat a = stage<R, CX>(A, st);
   std::unique_ptr<StagedMat> ul, ur;
   if (want_l) ul.reset(new StagedMat(UL.ptr, (i64)n, (i64)n, (i64)UL.row_stride, (i64)UL.col_stride, es, true, true, st));
   if (want_r) ur.reset(new StagedMat(UR.ptr, (i64)n, (i64)n, (i64)UR.row_stride, (i64)UR.col_stride, es, true, true, st));
@@ -448,8 +445,7 @@ FaerV0_24_EvdStatus evd_entry(FaerV0_24_MatRef A, FaerV0_24_MatMut UL, FaerV0_24
   if (ul) ul->finish();
   if (ur) ur->finish();
   ws_free(s_dev);
-  if (!ok) out.tag = FaerV0_24_EvdStatus_NoConvergence;
-  return out;
+  return evd_status(ok);
 }
 
 }  // namespace

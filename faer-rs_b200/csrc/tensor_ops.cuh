@@ -47,15 +47,15 @@ template <class T>
 inline View<const T> cview(const View<T>& v) { return View<const T>{v.ptr, v.nrows, v.ncols, v.rs, v.cs}; }
 
 // The same building blocks over the scalar kind <R, complex?>: <double, false> f64, <float, false> f32, <double, true> c64,
-// <float, true> c32 (complex views in COMPLEX element units on an R* base). Real kinds ignore the conjugation flags; complex
-// products take a real alpha.
+// <float, true> c32 (complex views in COMPLEX element units on an R* base). Real kinds ignore the conjugation flags and
+// `alpha_im`.
 template <class R, bool CX>
 inline void gemm_t(cudaStream_t st, View<R> dst, int ds, int accum, View<const R> lhs, int ls, bool conj_lhs, View<const R> rhs,
-                   int rs, bool conj_rhs, R alpha) {
-  if constexpr (std::is_same_v<R, dd>) gemm_dd(st, dst, ds, accum, lhs, ls, conj_lhs, rhs, rs, conj_rhs, CX, alpha, R(0));
+                   int rs, bool conj_rhs, R alpha, R alpha_im = R(0)) {
+  if constexpr (std::is_same_v<R, dd>) gemm_dd(st, dst, ds, accum, lhs, ls, conj_lhs, rhs, rs, conj_rhs, CX, alpha, alpha_im);
   else if constexpr (!CX) gemm(st, dst, ds, accum, lhs, ls, rhs, rs, alpha);
-  else if constexpr (sizeof(R) == 8) gemm_c64(st, dst, ds, accum, lhs, ls, conj_lhs, rhs, rs, conj_rhs, alpha, 0.0);
-  else gemm_c32(st, dst, ds, accum, lhs, ls, conj_lhs, rhs, rs, conj_rhs, alpha, 0.0f);
+  else if constexpr (sizeof(R) == 8) gemm_c64(st, dst, ds, accum, lhs, ls, conj_lhs, rhs, rs, conj_rhs, alpha, alpha_im);
+  else gemm_c32(st, dst, ds, accum, lhs, ls, conj_lhs, rhs, rs, conj_rhs, alpha, alpha_im);
 }
 template <class R, bool CX>
 inline void solve_lower_t(cudaStream_t st, View<const R> t, bool unit, bool conj, View<R> rhs) {
