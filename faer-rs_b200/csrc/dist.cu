@@ -200,83 +200,7 @@ static bool ensure_green_streams() {
   g_green_main = (cudaStream_t)s_main;
   g_green_urgent = (cudaStream_t)s_urgent;
   g_green_panel_sms = (int)grp[0].sm.smCount;
-  if (getenv("FAER_B200_VERBOSE"))
-    fprintf(stderr, "faer_b200: SM partition: %u SMs for the panel chain, %u for trailing updates\n", grp[0].sm.smCount,
-            rem.sm.smCount);
   g_green_state = 1;
-  return true;
-}
-
-// A second, independently sized partition for drivers whose panel kernel needs more SMs than the LU one (the QR panel
-// keeps its slices in shared memory: >= 42 CTAs at 65536 rows). Created on first use, one per requested size, never
-// resized. Used only by the opt-in look-ahead QR driver (qr.cu, FAER_B200_QR_LOOKAHEAD=<SMs>).
-bool partition_streams(int panel_sms, cudaStream_t* panel, cudaStream_t* urgent, cudaStream_t* bulk, int* got_panel_sms) {
-  struct Set {
-    int want;
-    int state;  // 0 = unused slot, 1 = ok, -1 = failed
-    cudaStream_t sp, su, sm;
-    int sms;
-  };
-  static Set sets[4] = {};
-  Set* s = nullptr;
-  for (auto& c : sets)
-    if (c.state != 0 && c.want == panel_sms) s = &c;
-  if (!s) {
-    for (auto& c : sets)
-      if (c.state == 0) {
-        s = &c;
-        break;
-      }
-    if (!s) return false;
-    s->want = panel_sms;
-    s->state = -1;
-    void* f[6] = {};
-    const char* names[6] = {"cuDeviceGet", "cuDeviceGetDevResource", "cuDevSmResourceSplitByCount", "cuDevResourceGenerateDesc",
-                            "cuGreenCtxCreate", "cuGreenCtxStreamCreate"};
-    for (int i = 0; i < 6; ++i) {
-      cudaDriverEntryPointQueryResult q;
-      if (cudaGetDriverEntryPoint(names[i], &f[i], cudaEnableDefault, &q) != cudaSuccess || !f[i]) return false;
-    }
-    auto p_get = (decltype(&cuDeviceGet))f[0];
-    auto p_res = (decltype(&cuDeviceGetDevResource))f[1];
-    auto p_split = (decltype(&cuDevSmResourceSplitByCount))f[2];
-    auto p_desc = (decltype(&cuDevResourceGenerateDesc))f[3];
-    auto p_ctx = (decltype(&cuGreenCtxCreate))f[4];
-    auto p_stream = (decltype(&cuGreenCtxStreamCreate))f[5];
-    int dev = 0;
-    FB_CUDA_CHECK(cudaGetDevice(&dev));
-    FB_CUDA_CHECK(cudaFree(0));
-    CUdevice cudev;
-    CUdevResource all, grp[1], rem;
-    unsigned int ngrp = 1;
-    CUdevResourceDesc d_panel, d_main;
-    CUgreenCtx g_panel, g_main;
-    CUstream sp, su, sm;
-    int lo = 0, hi = 0;
-    FB_CUDA_CHECK(cudaDeviceGetStreamPriorityRange(&lo, &hi));
-    if (p_get(&cudev, dev) != CUDA_SUCCESS || p_res(cudev, &all, CU_DEV_RESOURCE_TYPE_SM) != CUDA_SUCCESS ||
-        p_split(grp, &ngrp, &all, &rem, 0, (unsigned int)panel_sms) != CUDA_SUCCESS || ngrp < 1 ||
-        rem.type != CU_DEV_RESOURCE_TYPE_SM || rem.sm.smCount == 0 || p_desc(&d_panel, &grp[0], 1) != CUDA_SUCCESS ||
-        p_desc(&d_main, &rem, 1) != CUDA_SUCCESS || p_ctx(&g_panel, d_panel, cudev, CU_GREEN_CTX_DEFAULT_STREAM) != CUDA_SUCCESS ||
-        p_ctx(&g_main, d_main, cudev, CU_GREEN_CTX_DEFAULT_STREAM) != CUDA_SUCCESS ||
-        p_stream(&sp, g_panel, CU_STREAM_NON_BLOCKING, hi) != CUDA_SUCCESS ||
-        p_stream(&su, g_main, CU_STREAM_NON_BLOCKING, hi) != CUDA_SUCCESS ||
-        p_stream(&sm, g_main, CU_STREAM_NON_BLOCKING, lo) != CUDA_SUCCESS)
-      return false;
-    s->sp = (cudaStream_t)sp;
-    s->su = (cudaStream_t)su;
-    s->sm = (cudaStream_t)sm;
-    s->sms = (int)grp[0].sm.smCount;
-    s->state = 1;
-    register_stream_sms(s->sp, (int)grp[0].sm.smCount);
-    register_stream_sms(s->su, (int)rem.sm.smCount);
-    register_stream_sms(s->sm, (int)rem.sm.smCount);
-  }
-  if (s->state != 1) return false;
-  *panel = s->sp;
-  *urgent = s->su;
-  *bulk = s->sm;
-  *got_panel_sms = s->sms;
   return true;
 }
 
@@ -524,7 +448,7 @@ LltResult dist_llt_f64(double* A_local, i64 ld, i64 n, i64 nb, double reg_delta,
       }
       factor_and_bcast(kn);
     }
-    if (P == 1 && k + 2 < nblk && !(pipe && k == 0) && !getenv("FAER_B200_LLT_SPLIT_BULK")) {
+    if (P == 1 && k + 2 < nblk && !(pipe && k == 0)) {
       // single GPU: every remaining block column in ONE structured launch (lower-triangular destination: tiles above
       // the diagonal exit at once) instead of one launch per block column — no per-launch tail, better L2 reuse
       const i64 k0 = b0[(size_t)k], kb = b0[(size_t)k + 1] - k0, rows_k = n - k0, j0 = b0[(size_t)k + 2];
@@ -581,10 +505,8 @@ LltResult llt_host_pipelined_f64(double* hostA, i64 host_ld, i64 n, i64 nb, doub
     FB_CUDA_CHECK(cudaStreamCreateWithFlags(&s_h2d, cudaStreamNonBlocking));
     FB_CUDA_CHECK(cudaStreamCreateWithFlags(&s_d2h, cudaStreamNonBlocking));
   }
-  // the left-looking first half (opt-in) walks uniform blocks; the default path shares dist_llt_f64's boundaries
-  const char* hl0 = getenv("FAER_B200_HOST_LEFT");
-  const bool hybrid = hl0 && atoi(hl0) != 0;
-  const std::vector<i64> b0 = llt_block_bounds(n, nb, /*uniform*/ hybrid);
+  // the same block boundaries as dist_llt_f64, which waits for block column j at its first touch
+  const std::vector<i64> b0 = llt_block_bounds(n, nb, /*uniform*/ false);
   const i64 nblk = (i64)b0.size() - 1;
   double* dA = (double*)ws_alloc((size_t)n * n * 8);
   LltHostPipe pipe;
@@ -599,87 +521,9 @@ LltResult llt_host_pipelined_f64(double* hostA, i64 host_ld, i64 n, i64 nb, doub
                                     (size_t)(n - j0) * 8, (size_t)jb, cudaMemcpyHostToDevice, s_h2d));
     FB_CUDA_CHECK(cudaEventRecord(pipe.up[(size_t)j], s_h2d));
   }
-  // Hybrid order, OPT-IN (FAER_B200_HOST_LEFT=1): the left-looking half is bound by its own potrf / solve chain, so it
-  // is not the default. A right-looking factorization cannot get past its first step before
-  // the LAST block column has arrived (every step updates every column), i.e. it idles for as long as the whole upload
-  // takes. While the upload runs, the first half of the block columns is therefore factored LEFT-looking — column
-  // j only needs the panels to its left, so it is processed the moment it lands: one GEMM with k = j0 applies all previous
-  // panels, then potrf + solve, then the finished column goes home. When the upload is complete, one structured GEMM
-  // brings the trailing half up to date and the right-looking look-ahead driver (above) finishes it.
-  const i64 J = (hybrid && nblk >= 8) ? nblk / 2 : 0;
-  LltResult r{true, 0, 0};
-  if (J > 0) {
-    ensure_streams();
-    cudaStream_t sc = g_main_stream;
-    long long* d_info = (long long*)ws_alloc(4 * sizeof(long long));
-    long long h_info[2] = {-1, 0};
-    FB_CUDA_CHECK(cudaMemcpyAsync(d_info, h_info, sizeof(h_info), cudaMemcpyHostToDevice, sc));
-    std::vector<cudaEvent_t> ev_done((size_t)J);
-    for (i64 j = 0; j < J; ++j) {
-      const i64 j0 = j * nb, jb = std::min(nb, n - j0), below = n - j0 - jb;
-      FB_CUDA_CHECK(cudaStreamWaitEvent(sc, pipe.up[(size_t)j], 0));
-      VD djj{dA + j0 * n + j0, jb, jb, 1, n};
-      if (j > 0) {
-        VCD Lj{dA + j0, jb, j0, 1, n};  // rows of block j in the panels 0 .. j-1
-        gemm_f64(sc, djj, TRI_LOWER, 1, Lj, RECT, Lj.t(), RECT, -1.0);
-        if (below > 0) {
-          VCD Lb{dA + j0 + jb, below, j0, 1, n};
-          VD dbj{dA + j0 * n + j0 + jb, below, jb, 1, n};
-          gemm_f64(sc, dbj, 1, Lb, Lj.t(), -1.0);
-        }
-      }
-      llt_cholesky_device_f64(sc, djj, reg_delta, reg_eps, d_info, j0);
-      if (below > 0) {
-        VD bl{dA + j0 * n + j0 + jb, below, jb, 1, n};
-        solve_lower_triangular_in_place_f64(sc, cv(djj), false, bl.t());
-      }
-      FB_CUDA_CHECK(cudaEventCreateWithFlags(&ev_done[(size_t)j], cudaEventDisableTiming));
-      FB_CUDA_CHECK(cudaEventRecord(ev_done[(size_t)j], sc));
-      FB_CUDA_CHECK(cudaStreamWaitEvent(s_d2h, ev_done[(size_t)j], 0));
-      FB_CUDA_CHECK(cudaMemcpy2DAsync(hostA + j0 * host_ld + j0, (size_t)host_ld * 8, dA + j0 * n + j0, (size_t)n * 8,
-                                      (size_t)(n - j0) * 8, (size_t)jb, cudaMemcpyDeviceToHost, s_d2h));
-    }
-    // trailing half: all panels 0 .. J-1 at once (needs every remaining column on the device)
-    const i64 J0 = J * nb, nt = n - J0;
-    for (i64 j = J; j < nblk; ++j) FB_CUDA_CHECK(cudaStreamWaitEvent(sc, pipe.up[(size_t)j], 0));
-    {
-      VCD Lt{dA + J0, nt, J0, 1, n};
-      VD dt{dA + J0 * n + J0, nt, nt, 1, n};
-      gemm_f64(sc, dt, TRI_LOWER, 1, Lt, RECT, Lt.t(), RECT, -1.0);
-    }
-    FB_CUDA_CHECK(cudaMemcpyAsync(h_info, d_info, sizeof(h_info), cudaMemcpyDeviceToHost, sc));
-    cudaEvent_t ev_half;
-    FB_CUDA_CHECK(cudaEventCreateWithFlags(&ev_half, cudaEventDisableTiming));
-    FB_CUDA_CHECK(cudaEventRecord(ev_half, sc));
-    FB_CUDA_CHECK(cudaStreamWaitEvent(current_stream(), ev_half, 0));
-    // right-looking look-ahead driver on the trailing block; its finished panels go home through the same pipe
-    LltHostPipe tail;
-    tail.host = hostA + J0 * host_ld + J0;
-    tail.host_ld = host_ld;
-    tail.s_d2h = s_d2h;
-    tail.up.assign(llt_block_bounds(nt, nb, false).size(), pipe.up[(size_t)(nblk - 1)]);
-    g_llt_pipe = &tail;
-    LltResult rt = dist_llt_f64(dA + J0 * n + J0, n, nt, nb, reg_delta, reg_eps, /*lookahead | local*/ 3);
-    g_llt_pipe = nullptr;
-    FB_CUDA_CHECK(cudaStreamSynchronize(sc));
-    FB_CUDA_CHECK(cudaStreamSynchronize(s_d2h));
-    if (h_info[0] >= 0) {
-      r.ok = false;
-      r.non_positive_pivot_index = (size_t)h_info[0];
-    } else if (!rt.ok) {
-      r.ok = false;
-      r.non_positive_pivot_index = rt.non_positive_pivot_index + (size_t)J0;
-    } else {
-      r.dynamic_regularization_count = (size_t)h_info[1] + rt.dynamic_regularization_count;
-    }
-    for (i64 j = 0; j < J; ++j) cudaEventDestroy(ev_done[(size_t)j]);
-    cudaEventDestroy(ev_half);
-    ws_free(d_info);
-  } else {
-    g_llt_pipe = &pipe;
-    r = dist_llt_f64(dA, n, n, nb, reg_delta, reg_eps, /*lookahead | local*/ 3);
-    g_llt_pipe = nullptr;
-  }
+  g_llt_pipe = &pipe;
+  const LltResult r = dist_llt_f64(dA, n, n, nb, reg_delta, reg_eps, /*lookahead | local*/ 3);
+  g_llt_pipe = nullptr;
   FB_CUDA_CHECK(cudaStreamSynchronize(s_h2d));
   for (i64 j = 0; j < nblk; ++j) cudaEventDestroy(pipe.up[(size_t)j]);
   ws_free(dA);
@@ -694,44 +538,27 @@ LltResult llt_host_pipelined_f64(double* hostA, i64 host_ld, i64 n, i64 nb, doub
 // trailing-update CTAs occupied every SM; on its own partition it overlaps with the GEMMs completely.
 static void lu_local_partitioned_f64(double* A, i64 ld, i64 n, i64 nb, int* d_trans) {
   cudaStream_t sp = g_green_panel, su = g_green_urgent, sm = g_green_main;
-  const bool trace = getenv("FAER_B200_TRACE") != nullptr;
-  const unsigned evf = trace ? cudaEventDefault : cudaEventDisableTiming;
   cudaEvent_t ev_start;
-  FB_CUDA_CHECK(cudaEventCreateWithFlags(&ev_start, evf));
+  FB_CUDA_CHECK(cudaEventCreateWithFlags(&ev_start, cudaEventDisableTiming));
   FB_CUDA_CHECK(cudaEventRecord(ev_start, current_stream()));
   FB_CUDA_CHECK(cudaStreamWaitEvent(sp, ev_start, 0));
   FB_CUDA_CHECK(cudaStreamWaitEvent(su, ev_start, 0));
   FB_CUDA_CHECK(cudaStreamWaitEvent(sm, ev_start, 0));
-  // Block boundaries. FAER_B200_LU_WIDE=1 makes the blocks of the first half of the columns (where the schedule is
-  // bound by the trailing updates) twice as wide — deeper GEMMs, half the row-swap / TRSM passes; opt-in, uniform blocks are the
-  // default.
   std::vector<i64> b0;
-  {
-    const char* e = getenv("FAER_B200_LU_WIDE");
-    const bool wide = (e ? atoi(e) != 0 : false) && nb <= 512;
-    for (i64 c = 0; c < n;) {
-      b0.push_back(c);
-      c += (wide && 2 * c < n) ? std::min<i64>(2 * nb, n - c) : std::min<i64>(nb, n - c);
-    }
-    b0.push_back(n);
-  }
+  for (i64 c = 0; c < n; c += std::min<i64>(nb, n - c)) b0.push_back(c);
+  b0.push_back(n);
   const i64 nblk = (i64)b0.size() - 1;
-  const i64 nbmax = 2 * nb;
-  LuWorkspace* wp = lu_ws_create(sp, nbmax, g_green_panel_sms);
-  if (!getenv("FAER_B200_NO_OFFLOAD")) lu_ws_set_big_stream(wp, su);  // big recursion nodes run on the update partition
-  {
-    // leaves on a thread-block cluster (DSMEM exchange) inside the panel partition; FAER_B200_LU_CLUSTER=0 disables
-    const char* e = getenv("FAER_B200_LU_CLUSTER");
-    const int want = e ? atoi(e) : 16;
-    if (want > 0) lu_ws_set_cluster(wp, std::min(want, g_green_panel_sms >= 16 ? 16 : 8));
-  }
-  LuWorkspace* wu = lu_ws_create(su, nbmax);
-  LuWorkspace* wm = lu_ws_create(sm, nbmax);
+  LuWorkspace* wp = lu_ws_create(sp, nb, g_green_panel_sms);
+  lu_ws_set_big_stream(wp, su);  // big recursion nodes run on the update partition
+  // leaves on a thread-block cluster (DSMEM exchange) inside the panel partition
+  lu_ws_set_cluster(wp, g_green_panel_sms >= 16 ? 16 : 8);
+  LuWorkspace* wu = lu_ws_create(su, nb);
+  LuWorkspace* wm = lu_ws_create(sm, nb);
   std::vector<cudaEvent_t> ev_panel((size_t)nblk), ev_ready((size_t)nblk), ev_first((size_t)nblk);
   for (i64 k = 0; k < nblk; ++k) {
-    FB_CUDA_CHECK(cudaEventCreateWithFlags(&ev_panel[(size_t)k], evf));
-    FB_CUDA_CHECK(cudaEventCreateWithFlags(&ev_ready[(size_t)k], evf));
-    FB_CUDA_CHECK(cudaEventCreateWithFlags(&ev_first[(size_t)k], evf));
+    FB_CUDA_CHECK(cudaEventCreateWithFlags(&ev_panel[(size_t)k], cudaEventDisableTiming));
+    FB_CUDA_CHECK(cudaEventCreateWithFlags(&ev_ready[(size_t)k], cudaEventDisableTiming));
+    FB_CUDA_CHECK(cudaEventCreateWithFlags(&ev_first[(size_t)k], cudaEventDisableTiming));
   }
   auto factor_panel = [&](i64 k) {  // on sp
     const i64 k0 = b0[(size_t)k], kb = b0[(size_t)k + 1] - k0, rows = n - k0;
@@ -780,16 +607,6 @@ static void lu_local_partitioned_f64(double* A, i64 ld, i64 n, i64 nb, int* d_tr
   FB_CUDA_CHECK(cudaStreamSynchronize(sp));
   FB_CUDA_CHECK(cudaStreamSynchronize(su));
   FB_CUDA_CHECK(cudaStreamSynchronize(sm));
-  if (trace) {
-    auto at = [&](cudaEvent_t e) {
-      float ms = 0.f;
-      return cudaEventElapsedTime(&ms, ev_start, e) == cudaSuccess ? ms : -1.f;
-    };
-    fprintf(stderr, "LU n=%lld nb=%lld timeline (ms since start): k: col-ready panel-done bulk-first\n", n, nb);
-    for (i64 k = 0; k < nblk; ++k)
-      fprintf(stderr, "  %3lld: %8.3f %8.3f %8.3f\n", k, k ? at(ev_ready[(size_t)k]) : 0.f, at(ev_panel[(size_t)k]),
-              k + 2 < nblk ? at(ev_first[(size_t)k]) : -1.f);
-  }
   for (i64 k = 0; k < nblk; ++k) {
     cudaEventDestroy(ev_panel[(size_t)k]);
     cudaEventDestroy(ev_ready[(size_t)k]);
@@ -834,17 +651,15 @@ size_t dist_lu_f64(double* A_local, i64 ld, i64 n, i64 nb, long long* perm_fwd, 
   //   sm  bulk trailing updates                                                   sb  the NCCL broadcast (plain stream)
   // Without a partition (FAER_B200_GREEN_SMS=0 or no look-ahead) sp = su = sb is the high-priority stream.
   if (lookahead) ensure_streams();
-  const bool part = lookahead && !getenv("FAER_B200_DIST_NO_PARTITION") && ensure_green_streams();
+  const bool part = lookahead && ensure_green_streams();
   cudaStream_t sp = part ? g_green_panel : (lookahead ? g_panel_stream : current_stream());
   cudaStream_t su = part ? g_green_urgent : sp;
   cudaStream_t sm = part ? g_green_main : (lookahead ? g_main_stream : current_stream());
   cudaStream_t sb = part ? g_panel_stream : sp;
   const bool two_streams = sp != sm && lookahead;
   if (!two_streams) sm = sp;
-  const bool trace = getenv("FAER_B200_TRACE") != nullptr;
-  const unsigned evf = trace ? cudaEventDefault : cudaEventDisableTiming;
   cudaEvent_t ev_start;
-  FB_CUDA_CHECK(cudaEventCreateWithFlags(&ev_start, evf));
+  FB_CUDA_CHECK(cudaEventCreateWithFlags(&ev_start, cudaEventDisableTiming));
   FB_CUDA_CHECK(cudaEventRecord(ev_start, current_stream()));
   for (cudaStream_t st : {sp, su, sm, sb})
     if (st != current_stream()) FB_CUDA_CHECK(cudaStreamWaitEvent(st, ev_start, 0));
@@ -857,21 +672,19 @@ size_t dist_lu_f64(double* A_local, i64 ld, i64 n, i64 nb, long long* perm_fwd, 
   int* d_trans = (int*)ws_alloc((size_t)n * sizeof(int));
   LuWorkspace* wp = lu_ws_create(sp, nb, part ? g_green_panel_sms : 0);
   if (part) {
-    if (!getenv("FAER_B200_NO_OFFLOAD")) lu_ws_set_big_stream(wp, su);
-    const char* e = getenv("FAER_B200_LU_CLUSTER");
-    const int want = e ? atoi(e) : 16;
-    if (want > 0) lu_ws_set_cluster(wp, std::min(want, g_green_panel_sms >= 16 ? 16 : 8));
+    lu_ws_set_big_stream(wp, su);
+    lu_ws_set_cluster(wp, g_green_panel_sms >= 16 ? 16 : 8);
   }
   LuWorkspace* wu = (su != sp) ? lu_ws_create(su, nb) : wp;
   LuWorkspace* wm = two_streams ? lu_ws_create(sm, nb) : wp;
   std::vector<cudaEvent_t> ev_fact((size_t)nblk), ev_bcast((size_t)nblk), ev_used((size_t)nblk), ev_first((size_t)nblk),
       ev_ready((size_t)nblk);
   for (i64 k = 0; k < nblk; ++k) {
-    FB_CUDA_CHECK(cudaEventCreateWithFlags(&ev_fact[(size_t)k], evf));
-    FB_CUDA_CHECK(cudaEventCreateWithFlags(&ev_bcast[(size_t)k], evf));
-    FB_CUDA_CHECK(cudaEventCreateWithFlags(&ev_used[(size_t)k], evf));
-    FB_CUDA_CHECK(cudaEventCreateWithFlags(&ev_first[(size_t)k], evf));
-    FB_CUDA_CHECK(cudaEventCreateWithFlags(&ev_ready[(size_t)k], evf));
+    FB_CUDA_CHECK(cudaEventCreateWithFlags(&ev_fact[(size_t)k], cudaEventDisableTiming));
+    FB_CUDA_CHECK(cudaEventCreateWithFlags(&ev_bcast[(size_t)k], cudaEventDisableTiming));
+    FB_CUDA_CHECK(cudaEventCreateWithFlags(&ev_used[(size_t)k], cudaEventDisableTiming));
+    FB_CUDA_CHECK(cudaEventCreateWithFlags(&ev_first[(size_t)k], cudaEventDisableTiming));
+    FB_CUDA_CHECK(cudaEventCreateWithFlags(&ev_ready[(size_t)k], cudaEventDisableTiming));
   }
   // number of local columns that belong to blocks with index < b
   auto cols_before = [&](i64 b) {
@@ -979,20 +792,6 @@ size_t dist_lu_f64(double* A_local, i64 ld, i64 n, i64 nb, long long* perm_fwd, 
   FB_CUDA_CHECK(cudaStreamSynchronize(su));
   FB_CUDA_CHECK(cudaStreamSynchronize(sm));
   FB_CUDA_CHECK(cudaMemcpy(h_trans.data(), d_trans, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost));
-  if (trace && me == 0) {
-    auto at = [&](cudaEvent_t e) {
-      float ms = 0.f;
-      if (cudaEventElapsedTime(&ms, ev_start, e) == cudaSuccess) return ms;
-      (void)cudaGetLastError();
-      return -1.f;
-    };
-    fprintf(stderr, "dist LU n=%lld nb=%lld P=%d rank 0 timeline (ms): k: col-ready factored(owner) bcast-done bulk-first bulk-done\n",
-            n, nb, P);
-    for (i64 k = 0; k < nblk; ++k)
-      fprintf(stderr, "  %3lld: %8.3f %8.3f %8.3f %8.3f %8.3f\n", k, k ? at(ev_ready[(size_t)k]) : 0.f,
-              (int)(k % P) == me ? at(ev_fact[(size_t)k]) : -1.f, at(ev_bcast[(size_t)k]), at(ev_first[(size_t)k]),
-              at(ev_used[(size_t)k]));
-  }
   for (i64 i = 0; i < n; ++i) {
     const int t = h_trans[(size_t)i];
     if (t != 0) {

@@ -301,19 +301,11 @@ inline int f_transpose_struct(int s) {
 }
 inline bool f_aligned16(const void* p) { return (((uintptr_t)p) & 15) == 0; }
 
-// wgmma path switch (FAER_B200_F32_TC=0 keeps everything on the mma.sync kernel) and its per-stream packing workspace
-// (grow-only device buffers; work on one stream is ordered, so a stream's buffer can be reused call after call)
-bool f32_tc_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("FAER_B200_F32_TC");
-    v = e ? (atoi(e) != 0) : 1;
-  }
-  return v != 0;
-}
 // split-K partial buffer of the mma.sync kernel: per-stream grow-only scratch (runtime.cu)
 float* f32_split_workspace(cudaStream_t stream, size_t bytes) { return (float*)stream_scratch(stream, bytes); }
 
+// per-stream packing workspace of the wgmma path (grow-only device buffers; work on one stream is ordered, so a stream's
+// buffer can be reused call after call)
 tc::Workspace* f32_tc_workspace(cudaStream_t stream) {
   struct Slot {
     cudaStream_t st;
@@ -372,7 +364,7 @@ void gemm_f32(cudaStream_t stream, VF dst, int dst_struct, int accum, VCF lhs, i
   }
   // Large unstructured products go to the wgmma kernel (gemm_f32_tc.cuh: TMA + mbarrier pipeline, 3xTF32 on the Hopper
   // tensor cores). Structured operands / destinations and small products stay on the mma.sync kernel.
-  if (dst_struct == RECT && lhs_struct == RECT && rhs_struct == RECT && f32_tc_enabled() && dst.nrows >= 64 &&
+  if (dst_struct == RECT && lhs_struct == RECT && rhs_struct == RECT && dst.nrows >= 64 &&
       dst.ncols >= 64 && lhs.ncols >= 32 && 2.0 * (double)dst.nrows * (double)dst.ncols * (double)lhs.ncols >= 2.5e8) {
     tc::Operand a{lhs.ptr, (int)lhs.nrows, (int)lhs.ncols, lhs.rs, lhs.cs};
     tc::Operand b{rhs.ptr, (int)rhs.nrows, (int)rhs.ncols, rhs.rs, rhs.cs};

@@ -19,9 +19,8 @@ namespace fb {
 
 namespace {
 
-template <int WARPS_M_, int WARPS_N_, int WMI_, int WNI_, int BK_, int STAGES_, bool SWZ_ = false>
+template <int WARPS_M_, int WARPS_N_, int WMI_, int WNI_, int BK_, int STAGES_>
 struct TileCfg {
-  static constexpr bool SWZ = SWZ_;
   static constexpr int WARPS_M = WARPS_M_, WARPS_N = WARPS_N_, WMI = WMI_, WNI = WNI_, BK = BK_, STAGES = STAGES_;
   static constexpr int BM = WARPS_M * WMI * 8;
   static constexpr int BN = WARPS_N * WNI * 8;
@@ -30,26 +29,20 @@ struct TileCfg {
 
 // One operand tile: `ROWS` indices along the non-contracted dim (mn) x BK along k.
 // KMAJOR: smem[mn][k] (ld = BK+4) else smem[k][mn] (ld = ROWS+4).
-// SWZ = false: rows padded by 4 doubles. SWZ = true (BK == 16 only): dense tile with an XOR swizzle of bits 2..3 of
-// the fast index by the low two bits of the slow index — the same 16 distinct 8-byte banks per half-warp fragment
-// load, 20 % less shared memory (=> one more resident CTA per SM). 16-byte cp.async chunks stay contiguous
-// (the XOR only touches bits >= 2 of the element index).
-template <int ROWS, int BK, bool KMAJOR, bool SWZ = false>
+template <int ROWS, int BK, bool KMAJOR>
 struct OpTile {
-  static_assert(!SWZ || BK == 16, "swizzled tiles need BK == 16");
-  static constexpr int LD = SWZ ? (KMAJOR ? BK : ROWS) : (KMAJOR ? BK + 4 : ROWS + 4);
+  static constexpr int LD = KMAJOR ? BK + 4 : ROWS + 4;
   static constexpr int SIZE = KMAJOR ? ROWS * LD : BK * LD;
   __device__ static __forceinline__ int idx(int mn, int kk) {
-    if constexpr (SWZ) return KMAJOR ? mn * LD + (kk ^ ((mn & 3) << 2)) : kk * LD + (mn ^ ((kk & 3) << 2));
     return KMAJOR ? mn * LD + kk : kk * LD + mn;
   }
 };
 
 // Global -> shared copy of one operand tile. Element (mn, kk) lives at g + (mn0+mn)*s_mn + (k0+kk)*s_k.
-template <int ROWS, int BK, bool KMAJOR, bool VEC, int THREADS, bool SWZ>
+template <int ROWS, int BK, bool KMAJOR, bool VEC, int THREADS>
 __device__ __forceinline__ void load_tile(double* __restrict__ s, const double* __restrict__ g, i64 s_mn, i64 s_k,
                                           int mn0, int k0, int MN, int K, int tid) {
-  using T = OpTile<ROWS, BK, KMAJOR, SWZ>;
+  using T = OpTile<ROWS, BK, KMAJOR>;
   if constexpr (VEC) {
     constexpr int CHUNKS = ROWS * BK / 2;
     static_assert(CHUNKS % THREADS == 0, "tile/threads mismatch");
@@ -98,9 +91,9 @@ __device__ __forceinline__ void load_tile(double* __restrict__ s, const double* 
 // rel > 0 : kept side of a lower-triangular operand; rel == 0 : diagonal.
 // lhs (m x k): row = mn, col = k  -> rel_lower = mn - k
 // rhs (k x n): row = k,  col = mn -> rel_lower = k - mn
-template <int ROWS, int BK, bool KMAJOR, int THREADS, bool SWZ>
+template <int ROWS, int BK, bool KMAJOR, int THREADS>
 __device__ __forceinline__ void fixup_tile(double* s, int structure, bool is_rhs, int mn0, int k0, int tid) {
-  using T = OpTile<ROWS, BK, KMAJOR, SWZ>;
+  using T = OpTile<ROWS, BK, KMAJOR>;
   const bool lower = is_lower(structure);
   const double diagval = is_unit(structure) ? 1.0 : 0.0;
   const bool keepdiag = !(is_unit(structure) || is_strict(structure));
@@ -141,10 +134,9 @@ template <class Cfg, bool AK, bool BNM, bool VEC>
 __global__ void __launch_bounds__(Cfg::THREADS) gemm_f64_kernel(const GemmF64Params p) {
   constexpr int BM = Cfg::BM, BN = Cfg::BN, BK = Cfg::BK, STAGES = Cfg::STAGES, THREADS = Cfg::THREADS;
   constexpr int WMI = Cfg::WMI, WNI = Cfg::WNI;
-  constexpr bool SWZ = Cfg::SWZ;
   static_assert(BK == 16 && WMI % 2 == 0, "the main loop issues 16 x 8 x 16 DMMAs");
-  using TA = OpTile<BM, BK, AK, SWZ>;
-  using TB = OpTile<BN, BK, !BNM, SWZ>;  // rhs: K-major when b_rs == 1
+  using TA = OpTile<BM, BK, AK>;
+  using TB = OpTile<BN, BK, !BNM>;  // rhs: K-major when b_rs == 1
   extern __shared__ __align__(16) double smem[];
   double* As = smem;
   double* Bs = smem + STAGES * TA::SIZE;
@@ -198,8 +190,8 @@ __global__ void __launch_bounds__(Cfg::THREADS) gemm_f64_kernel(const GemmF64Par
 
   auto load_stage = [&](int stage, int kt) {
     const int k0 = k_begin + kt * BK;
-    load_tile<BM, BK, AK, VEC, THREADS, SWZ>(As + stage * TA::SIZE, p.A, p.a_rs, p.a_cs, m0, k0, p.m, p.k, tid);
-    load_tile<BN, BK, !BNM, VEC, THREADS, SWZ>(Bs + stage * TB::SIZE, p.B, p.b_cs, p.b_rs, n0, k0, p.n, p.k, tid);
+    load_tile<BM, BK, AK, VEC, THREADS>(As + stage * TA::SIZE, p.A, p.a_rs, p.a_cs, m0, k0, p.m, p.k, tid);
+    load_tile<BN, BK, !BNM, VEC, THREADS>(Bs + stage * TB::SIZE, p.B, p.b_cs, p.b_rs, n0, k0, p.n, p.k, tid);
   };
 
 #pragma unroll
@@ -219,8 +211,8 @@ __global__ void __launch_bounds__(Cfg::THREADS) gemm_f64_kernel(const GemmF64Par
       const bool fa = tile_needs_fixup(p.a_struct, false, m0, BM, k0, BK);
       const bool fb_ = tile_needs_fixup(p.b_struct, true, n0, BN, k0, BK);
       if (fa || fb_) {
-        if (fa) fixup_tile<BM, BK, AK, THREADS, SWZ>(a_s, p.a_struct, false, m0, k0, tid);
-        if (fb_) fixup_tile<BN, BK, !BNM, THREADS, SWZ>(b_s, p.b_struct, true, n0, k0, tid);
+        if (fa) fixup_tile<BM, BK, AK, THREADS>(a_s, p.a_struct, false, m0, k0, tid);
+        if (fb_) fixup_tile<BN, BK, !BNM, THREADS>(b_s, p.b_struct, true, n0, k0, tid);
         __syncthreads();
       }
     }
@@ -291,26 +283,12 @@ __global__ void __launch_bounds__(Cfg::THREADS) gemm_f64_kernel(const GemmF64Par
   }
 }
 
-using CfgL = TileCfg<2, 4, 8, 4, 16, 4>;   // 128 x 128 x 16, 256 threads, warp tile 64 x 32
-using CfgS = TileCfg<2, 2, 4, 4, 16, 4>;   // 64 x 64 x 16, 128 threads, warp tile 32 x 32
-using CfgS3 = TileCfg<2, 2, 4, 4, 16, 3>;  // 64 x 64 x 16, 3 stages (57 KB => 3 CTAs/SM)
-using CfgZ4 = TileCfg<2, 2, 4, 4, 16, 4, true>;  // 64 x 64 x 16 swizzled, 4 stages (64 KB; 3 CTAs/SM by shared memory,
-                                                 // 2 in the layout variants that need more than 168 registers)
-
-// development knob: FAER_B200_GEMM_CFG=1..10 forces one tile configuration (0/unset = heuristic)
-inline int forced_cfg() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("FAER_B200_GEMM_CFG");
-    v = e ? atoi(e) : 0;
-  }
-  return v;
-}
+using CfgS3 = TileCfg<2, 2, 4, 4, 16, 3>;  // 64 x 64 x 16, 128 threads, warp tile 32 x 32, 3 stages (57 KB => 3 CTAs/SM)
 
 template <class Cfg, bool AK, bool BNM>
 constexpr size_t smem_bytes() {
   return sizeof(double) * Cfg::STAGES *
-         (OpTile<Cfg::BM, Cfg::BK, AK, Cfg::SWZ>::SIZE + OpTile<Cfg::BN, Cfg::BK, !BNM, Cfg::SWZ>::SIZE);
+         (OpTile<Cfg::BM, Cfg::BK, AK>::SIZE + OpTile<Cfg::BN, Cfg::BK, !BNM>::SIZE);
 }
 
 template <class Cfg, bool AK, bool BNM, bool VEC>
@@ -333,17 +311,7 @@ void launch_cfg(cudaStream_t stream, GemmF64Params& p) {
 
 template <bool AK, bool BNM, bool VEC>
 void launch_layout(cudaStream_t stream, GemmF64Params& p) {
-  long long tiles_l = (long long)((p.m + 127) / 128) * ((p.n + 127) / 128);
-  if (is_lower(p.c_struct) || is_upper(p.c_struct)) tiles_l = tiles_l / 2 + 1;
-  switch (forced_cfg()) {
-    case 1: launch_cfg<CfgL, AK, BNM, VEC>(stream, p); return;
-    case 4: launch_cfg<CfgS, AK, BNM, VEC>(stream, p); return;
-    case 5: launch_cfg<CfgS3, AK, BNM, VEC>(stream, p); return;
-    case 10: launch_cfg<CfgZ4, AK, BNM, VEC>(stream, p); return;
-    default: break;
-  }
   // the 64x64 tile with several CTAs per SM: the prologue / epilogue of one CTA overlap another CTA's main loop
-  (void)tiles_l;
   launch_cfg<CfgS3, AK, BNM, VEC>(stream, p);
 }
 

@@ -191,20 +191,17 @@ __device__ __forceinline__ uint32_t off_k_major(int mn, int kk) {
   return (uint32_t)(mn * 128 + ((((kk >> 1) ^ (mn & 7)) << 4) | ((kk & 1) << 3)));
 }
 
-// VAR (bring-up variants, selected by FAER_B200_WS_VAR): 0 = production; 1 = no setmaxnreg, one CTA per SM; 5 = the kernel as
-// first written (no proxy fence before a stage is released, old dst values through L1), kept to reproduce the failure below.
-//
 // Stage release. The consumers read a stage with ld.shared (generic proxy) and the producer's next TMA load overwrites it
 // through the async proxy: a write-after-read ACROSS proxies, which the mbarrier hand-over alone does not order. Without
 // `fence.proxy.async` before the arrive on `empty[s]`, a warp can read B fragments the next load has already replaced. The old values of dst are read with ld.global.cg:
 // they are used once, and keeping them out of L1 leaves it to nothing at all (the operands arrive by TMA).
-template <bool WIDE, bool A_KMAJOR, bool B_KMAJOR, bool SPICY, int VAR = 0>
-__global__ void __launch_bounds__(Shape<WIDE>::THREADS, (VAR == 1 || WIDE) ? 1 : 2)  // re-divided below with setmaxnreg
+template <bool WIDE, bool A_KMAJOR, bool B_KMAJOR, bool SPICY>
+__global__ void __launch_bounds__(Shape<WIDE>::THREADS, WIDE ? 1 : 2)  // re-divided below with setmaxnreg
 gemm_f64_ws_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
                    const __grid_constant__ CUtensorMap mapC, const Params p) {
   using S = Shape<WIDE>;
   constexpr int BN = S::BN, STAGES = S::STAGES, STAGE_BYTES = S::STAGE_BYTES, CONSUMERS = S::CONSUMERS;
-  static_assert(!(WIDE && (SPICY || VAR != 0)), "the wide configuration has no spicy or bring-up variants");
+  static_assert(!(WIDE && SPICY), "the wide configuration has no spicy variant");
   extern __shared__ uint8_t ws_smem_raw[];
   const uint32_t smem_base = (smem_u32(ws_smem_raw) + 1023u) & ~1023u;
   uint8_t* smem_gen = ws_smem_raw + (smem_base - smem_u32(ws_smem_raw));
@@ -243,7 +240,7 @@ gemm_f64_ws_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
 
   if (warp < 4) {
     // ================= producer warpgroup =================
-    if constexpr (VAR != 1) asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(S::PRODUCER_REGS));
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(S::PRODUCER_REGS));
     if (warp == 0 && lane == 0) {
       uint32_t it = 0;  // global k-step counter: stage = it % STAGES, phase = (it / STAGES) & 1
       uint32_t ds = 0;  // staged tiles so far
@@ -312,7 +309,7 @@ gemm_f64_ws_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
   }
 
   // ================= consumer warpgroups =================
-  if constexpr (VAR != 1) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(S::CONSUMER_REGS));
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(S::CONSUMER_REGS));
   const int cw = warp - 4;
   const int g = lane >> 2, t = lane & 3;
   const int wm0 = (cw & 3) * (WMI * 8), wn0 = (cw >> 2) * (WNI * 8);  // warp tile rows [wm0, wm0 + 32) x cols [wn0, wn0 + 64)
@@ -408,7 +405,7 @@ gemm_f64_ws_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
             dmma1688(acc[2 * ip][j][0], acc[2 * ip][j][1], acc[2 * ip + 1][j][0], acc[2 * ip + 1][j][1], a[ip], b);
         }
       }
-      if constexpr (VAR != 5) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
       __syncwarp();
       if (lane == 0) mbar_arrive(&empty[s]);
     }
@@ -470,8 +467,7 @@ gemm_f64_ws_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
           const int col = n0 + wn0 + j * 8 + 2 * t + e;
-          if constexpr (VAR != 5) dst[j][e] = kept(row, col) ? __ldcg(p.C + roff + coloff(col)) : 0.0;
-          else dst[j][e] = kept(row, col) ? p.C[roff + coloff(col)] : 0.0;
+          dst[j][e] = kept(row, col) ? __ldcg(p.C + roff + coloff(col)) : 0.0;
         }
     };
     if (add) load_old(0, cv[0]);
@@ -605,25 +601,11 @@ inline bool try_gemm_f64_ws(cudaStream_t stream, const GemmF64Params& q, const S
     }
   }
   const int grid = (int)((tiles + p.tiles_per_cta - 1) / p.tiles_per_cta);
-  {
-    static int stagger = -1;
-    if (stagger < 0) {
-      const char* e = getenv("FAER_B200_WS_STAGGER");  // 0 switches the stagger off (dev knob)
-      stagger = e ? atoi(e) : 1;
-    }
-    // narrow only (two CTAs per SM): half a tile at the full rate of one SM, (k / 16) k-steps x 128 x 64 x 16 FMA /
-    // (128 FMA / clock) / 2
-    p.stagger_cycles = (!wide && stagger && grid >= 2 * p.sm_slots) ? (long long)((q.k + BK - 1) / BK) * 512 : 0;
-  }
+  // narrow only (two CTAs per SM): half a tile at the full rate of one SM, (k / 16) k-steps x 128 x 64 x 16 FMA /
+  // (128 FMA / clock) / 2
+  p.stagger_cycles = (!wide && grid >= 2 * p.sm_slots) ? (long long)((q.k + BK - 1) / BK) * 512 : 0;
   // one opt-in to > 48 KB of dynamic shared memory per kernel variant
-  static bool configured[20] = {};
-  static int var = -1, extra_smem = 0;
-  if (var < 0) {
-    const char* e = getenv("FAER_B200_WS_VAR");  // bring-up knob
-    var = e ? atoi(e) : 0;
-    const char* x = getenv("FAER_B200_WS_EXTRA_SMEM");  // bring-up knob: > 14 KB forces one CTA per SM
-    extra_smem = x ? atoi(x) : 0;
-  }
+  static bool configured[12] = {};
   auto launch = [&](int which, auto kern, int threads, int smem_bytes) {
     if (!configured[which]) {
       FB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
@@ -633,15 +615,12 @@ inline bool try_gemm_f64_ws(cudaStream_t stream, const GemmF64Params& q, const S
   };
   using N = Shape<false>;
   using W = Shape<true>;
-  const int nsm = N::SMEM_BYTES + extra_smem;
+  const int nsm = N::SMEM_BYTES;
   if (wide) {
-    if (ak && bk) launch(16, gemm_f64_ws_kernel<true, true, true, false>, W::THREADS, W::SMEM_BYTES);
-    else if (ak && !bk) launch(17, gemm_f64_ws_kernel<true, true, false, false>, W::THREADS, W::SMEM_BYTES);
-    else if (!ak && bk) launch(18, gemm_f64_ws_kernel<true, false, true, false>, W::THREADS, W::SMEM_BYTES);
-    else launch(19, gemm_f64_ws_kernel<true, false, false, false>, W::THREADS, W::SMEM_BYTES);
-  } else if (!sp && var != 0 && !ak) {
-    if (var == 1) { if (bk) launch(8, gemm_f64_ws_kernel<false, false, true, false, 1>, N::THREADS, nsm); else launch(9, gemm_f64_ws_kernel<false, false, false, false, 1>, N::THREADS, nsm); }
-    else { if (bk) launch(10, gemm_f64_ws_kernel<false, false, true, false, 5>, N::THREADS, nsm); else launch(11, gemm_f64_ws_kernel<false, false, false, false, 5>, N::THREADS, nsm); }
+    if (ak && bk) launch(8, gemm_f64_ws_kernel<true, true, true, false>, W::THREADS, W::SMEM_BYTES);
+    else if (ak && !bk) launch(9, gemm_f64_ws_kernel<true, true, false, false>, W::THREADS, W::SMEM_BYTES);
+    else if (!ak && bk) launch(10, gemm_f64_ws_kernel<true, false, true, false>, W::THREADS, W::SMEM_BYTES);
+    else launch(11, gemm_f64_ws_kernel<true, false, false, false>, W::THREADS, W::SMEM_BYTES);
   } else if (!sp) {
     if (ak && bk) launch(0, gemm_f64_ws_kernel<false, true, true, false>, N::THREADS, nsm);
     else if (ak && !bk) launch(1, gemm_f64_ws_kernel<false, true, false, false>, N::THREADS, nsm);

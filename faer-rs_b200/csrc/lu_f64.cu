@@ -610,7 +610,9 @@ __global__ void __launch_bounds__(SP_THREADS) lu_subpanel_cluster_kernel(double*
   namespace cg = cooperative_groups;
   cg::cluster_group cluster = cg::this_cluster();
   const int C = (int)cluster.num_blocks(), rank = (int)cluster.block_rank();
-  // dev aid: cycle counts per phase, accumulated by thread 0 of CTA 0 (prof == nullptr in production)
+  // Cycle counts per phase, accumulated by thread 0 of CTA 0 when prof != nullptr. The host always passes nullptr; the
+  // counters stay because the branches they add shape ptxas's register allocation: without them the <32, 1> instantiation
+  // spills ~44 KB and f64 LU at n = 8192 takes 145 ms instead of 50 ms (H100 80GB HBM3, 700 W).
   __shared__ long long pt[9];  // [8] = time of the last tick
   const bool profiling = prof != nullptr && rank == 0 && threadIdx.x == 0;
   if (profiling)
@@ -1047,17 +1049,6 @@ struct LuCtx {
 
 constexpr i64 PANEL_SMEM_BUDGET = 200 * 1024;
 
-// Upper bound on the CTAs of one cooperative panel launch. Fewer CTAs than SMs leave room for the trailing-update GEMM
-// of the look-ahead schedule to run next to the (latency-bound) panel; env FAER_B200_LU_PANEL_CTAS overrides.
-int panel_cta_cap(int num_sms) {
-  static int cap = -1;
-  if (cap < 0) {
-    const char* e = getenv("FAER_B200_LU_PANEL_CTAS");
-    cap = e ? atoi(e) : 0;
-  }
-  return cap > 0 ? std::min(cap, num_sms) : num_sms;
-}
-
 // widest window (<= PANEL_W) whose row slices (ceil(m / #CTAs) rows x (w|1) doubles) fit in shared memory
 constexpr i64 CL_SMEM_BUDGET = 200 * 1024;
 int cluster_width_for(int C, i64 m) {
@@ -1072,8 +1063,7 @@ int panel_width_for(const LuCtx& ctx, i64 m) {
     const int wc = cluster_width_for(ctx.cluster_ctas, m);
     if (wc >= 4) return wc;
   }
-  const int cap = panel_cta_cap(ctx.num_sms);
-  const i64 rows = std::max<i64>(1, (m + cap - 1) / cap);
+  const i64 rows = std::max<i64>(1, (m + ctx.num_sms - 1) / ctx.num_sms);
   i64 w = PANEL_SMEM_BUDGET / (8 * rows) - 1;
   if (w > PANEL_W) w = PANEL_W;
   if (w >= 16) w = w / 16 * 16;
@@ -1121,48 +1111,14 @@ bool launch_panel_cluster(LuCtx& ctx, VD P, int* trans, bool want_plan) {
   return true;
 }
 
-// dev aid (FAER_B200_LU_SUBPANEL_PROF=1): 8 cycle counters accumulated by the fused sub-panel kernel, printed at exit
-long long* g_subpanel_prof = nullptr;
-void subpanel_prof_report() {
-  if (!g_subpanel_prof) return;
-  long long h[8];
-  if (cudaMemcpy(h, g_subpanel_prof, sizeof(h), cudaMemcpyDeviceToHost) != cudaSuccess) return;
-  const char* names[8] = {"S1 load+crout", "S2 reduce+publish", "S2 cluster.sync", "S2 scan+swap+update", "store+plan+sync A",
-                          "S3 swaps", "S4 + syncs B,C", "-"};
-  fprintf(stderr, "faer_b200: fused LU sub-panel cycles (CTA 0 thread 0, all launches):");
-  for (int i = 0; i < 7; ++i) fprintf(stderr, "  %s %.3f Mcyc", names[i], (double)h[i] * 1e-6);
-  fprintf(stderr, "\n");
-}
-
-// Fused sub-panel (one cluster launch for the whole window); returns false when it does not apply here.
-int subpanel_max_width() {
-  static int w = -1;
-  if (w < 0) {
-    const char* e = getenv("FAER_B200_LU_FUSED_W");  // 0 disables the fused sub-panel kernel
-    w = e ? atoi(e) : 128;
-    if (w > SP_MAXW) w = SP_MAXW;
-  }
-  return w;
-}
-
-i64 subpanel_tall_rows() {
-  static i64 v = -1;
-  if (v < 0) {
-    const char* e = getenv("FAER_B200_LU_FUSED_TALL");  // dev knob: rows above which the fused width is halved
-    v = e ? atoll(e) : 16384;
-  }
-  return v;
-}
+// Fused sub-panel (one cluster launch for the whole window): the widest sub-panel it takes, and the rows above which that
+// width is halved
+constexpr i64 SUBPANEL_MAX_W = 128, SUBPANEL_TALL_ROWS = 16384;
 
 template <int WW, int R>
 cudaError_t launch_subpanel_t(LuCtx& ctx, VD P, int* trans, int rows_per_cta, size_t smem, bool want_plan) {
   const int C = ctx.cluster_ctas;
   static bool configured = false;
-  if (!g_subpanel_prof && getenv("FAER_B200_LU_SUBPANEL_PROF")) {
-    FB_CUDA_CHECK(cudaMalloc(&g_subpanel_prof, 64));
-    FB_CUDA_CHECK(cudaMemset(g_subpanel_prof, 0, 64));
-    atexit(subpanel_prof_report);
-  }
   if (!configured) {
     FB_CUDA_CHECK(cudaFuncSetAttribute(lu_subpanel_cluster_kernel<WW, R>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
     FB_CUDA_CHECK(cudaFuncSetAttribute(lu_subpanel_cluster_kernel<WW, R>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
@@ -1183,19 +1139,20 @@ cudaError_t launch_subpanel_t(LuCtx& ctx, VD P, int* trans, int rows_per_cta, si
   double* Aptr = P.ptr;
   i64 rs = P.rs, cs = P.cs;
   int m = (int)P.nrows, W = (int)P.ncols;
-  long long* prof = g_subpanel_prof;
   int* pr = want_plan ? ctx.plan_rows : nullptr;
+  long long* prof = nullptr;
   return cudaLaunchKernelEx(&cfg, lu_subpanel_cluster_kernel<WW, R>, Aptr, rs, cs, m, W, rows_per_cta, trans, pr, ctx.plan_src,
                             ctx.plan_cnt, prof);
 }
 
+// returns false when the fused sub-panel does not apply here
 bool launch_subpanel(LuCtx& ctx, VD P, int* trans, bool want_plan) {
   const int C = ctx.cluster_ctas;
   const i64 m = P.nrows, W = P.ncols;
   // tall panels: the Crout pass streams the CTA's rows of the earlier columns from L2 once per window (8-column windows above
   // 16384 rows), a cost per column proportional to the fused width: halve it there and let the recursion's GEMM (on the large
   // partition) supply the level above
-  const i64 wmax = (m > subpanel_tall_rows()) ? std::max<i64>(32, subpanel_max_width() / 2) : subpanel_max_width();
+  const i64 wmax = m > SUBPANEL_TALL_ROWS ? SUBPANEL_MAX_W / 2 : SUBPANEL_MAX_W;
   if (C <= 0 || W > wmax || W > m) return false;
   const int rows_per_cta = (int)((m + C - 1) / C);
   // R rows x WW columns per thread in registers (R * WW = 32): the smallest R whose 512 R rows cover the CTA's slice
@@ -1218,7 +1175,7 @@ bool launch_subpanel(LuCtx& ctx, VD P, int* trans, bool want_plan) {
 void launch_panel(LuCtx& ctx, VD P, int* trans, bool want_plan) {
   if (launch_panel_cluster(ctx, P, trans, want_plan)) return;
   const int m = (int)P.nrows, w = (int)P.ncols;
-  int G = (int)std::min<i64>(panel_cta_cap(ctx.num_sms), (m + 63) / 64);
+  int G = (int)std::min<i64>(ctx.num_sms, (m + 63) / 64);
   if (G < 1) G = 1;
   int rows_per_cta = (m + G - 1) / G;
   size_t smem = (size_t)rows_per_cta * (size_t)(w | 1) * sizeof(double);
@@ -1329,7 +1286,6 @@ size_t lu_partial_piv_in_place_f64(cudaStream_t stream, VD A, void* perm_fwd, vo
     FB_CUDA_CHECK(cudaGetDevice(&dev));
     FB_CUDA_CHECK(cudaDeviceGetAttribute(&ctx.num_sms, cudaDevAttrMultiProcessorCount, dev));
     ctx.recursion_threshold = (i64)params.recursion_threshold;
-    if (const char* e = getenv("FAER_B200_LU_CLUSTER")) ctx.cluster_ctas = std::min(atoi(e), CL_MAXC);  // dev knob
     const int G = ctx.num_sms;
     const i64 ngroups_max = (size + SWAP_GROUP - 1) / SWAP_GROUP + 1;
     ctx.d_trans = (int*)ws_alloc((size_t)size * sizeof(int));

@@ -474,141 +474,6 @@ i64 qr_recommended_block_size(i64 nrows, i64 ncols) {
   return std::max<i64>(1, std::min(bs, size));
 }
 
-// ---- look-ahead driver on a partitioned GPU (OPT-IN: FAER_B200_QR_LOOKAHEAD=<panel SMs>). Parity-green on hardware, but
-// the panel kernel loses more from running on part of the SMs than the overlap returns at 65536 x 4096 f32, so it is
-// kept opt-in. ------------------------------------------------------------------------------------------------
-// With the block applies on the wgmma GEMM the f32 QR is panel-bound (qr_panel_kernel). Same
-// schedule as lu_local_partitioned_f64 (dist.cu): the panel partition factors block j+1 (sub-panels, their T blocks, the
-// in-block applies) while the update partition applies block j's reflector to the columns right of block j+1; block j+1
-// itself is updated first, on the urgent stream. The panel kernel keeps its slices in shared memory, so the partition
-// must hold ceil(rows * 33 * sizeof(T) / 200 KB) CTAs: 48 SMs for 65536 x 32 f32.
-bool partition_streams(int panel_sms, cudaStream_t* panel, cudaStream_t* urgent, cudaStream_t* bulk, int* got_panel_sms);
-
-template <class T>
-static i64 qr_in_place_lookahead(cudaStream_t st, View<T> A, View<T> H, cudaStream_t sp, cudaStream_t su, cudaStream_t sm,
-                                 int panel_sms) {
-  const i64 m = A.nrows, n = A.ncols, size = std::min(m, n), bs = H.nrows;
-  const i64 nblk = (size + bs - 1) / bs;
-  const int Gmax = std::min(panel_sms, 160);
-  const size_t part_elems = (size_t)2 * Gmax * QR_NV, rowv_elems = (size_t)2 * QR_PW;
-  char* scb = (char*)ws_alloc((part_elems + rowv_elems + QR_PW) * sizeof(T) + 64);
-  QrScratch<T> sc;
-  sc.part = (T*)scb;
-  sc.rowv = sc.part + part_elems;
-  T* above2 = sc.rowv + rowv_elems;
-  sc.bar = (unsigned long long*)(((uintptr_t)(above2 + QR_PW) + 15) & ~(uintptr_t)15);
-  int* d_flag = (int*)ws_alloc(sizeof(int) * 4);
-  T* tmp_sp = (T*)ws_alloc((size_t)bs * bs * sizeof(T));
-  T* tmp_su = (T*)ws_alloc((size_t)bs * bs * sizeof(T));
-  T* tmp_sm = (T*)ws_alloc((size_t)bs * (size_t)n * sizeof(T));
-  cudaEvent_t ev_start;
-  FB_CUDA_CHECK(cudaEventCreateWithFlags(&ev_start, cudaEventDisableTiming));
-  FB_CUDA_CHECK(cudaEventRecord(ev_start, st));
-  FB_CUDA_CHECK(cudaStreamWaitEvent(sp, ev_start, 0));
-  FB_CUDA_CHECK(cudaStreamWaitEvent(su, ev_start, 0));
-  FB_CUDA_CHECK(cudaStreamWaitEvent(sm, ev_start, 0));
-  FB_CUDA_CHECK(cudaMemsetAsync(sc.bar, 0, 8, sp));
-  FB_CUDA_CHECK(cudaMemsetAsync(d_flag, 0, sizeof(int), sp));
-  unsigned long long bar_count = 0;
-  static bool configured = false;
-  if (!configured) {
-    FB_CUDA_CHECK(cudaFuncSetAttribute(qr_panel_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    configured = true;
-  }
-  std::vector<cudaEvent_t> ev_block((size_t)nblk), ev_ready((size_t)nblk), ev_first((size_t)nblk);
-  for (i64 j = 0; j < nblk; ++j) {
-    FB_CUDA_CHECK(cudaEventCreateWithFlags(&ev_block[(size_t)j], cudaEventDisableTiming));
-    FB_CUDA_CHECK(cudaEventCreateWithFlags(&ev_ready[(size_t)j], cudaEventDisableTiming));
-    FB_CUDA_CHECK(cudaEventCreateWithFlags(&ev_first[(size_t)j], cudaEventDisableTiming));
-  }
-  auto factor_block = [&](i64 jblk) {  // on sp: sub-panels, their T blocks, in-block applies, full T of the block
-    const i64 j0 = jblk * bs, jb = std::min(bs, size - j0);
-    for (i64 s0 = 0; s0 < jb; s0 += QR_PW) {
-      const i64 sw = std::min<i64>(QR_PW, jb - s0), c0 = j0 + s0;
-      const i64 mp = m - c0;
-      if (c0 > 0) {
-        col_sumsq_kernel<T><<<(unsigned)sw, 256, 0, sp>>>(A.at(0, c0), A.rs, A.cs, c0, above2);
-        FB_CUDA_CHECK(cudaGetLastError());
-        note_launch();
-      } else {
-        FB_CUDA_CHECK(cudaMemsetAsync(above2, 0, QR_PW * sizeof(T), sp));
-      }
-      int G = (int)std::min<i64>(Gmax, (mp + 63) / 64);
-      if (G < 1) G = 1;
-      int rows_per_cta = (int)((mp + G - 1) / G);
-      const size_t smem = (size_t)rows_per_cta * (size_t)((int)sw | 1) * sizeof(T);
-      FB_ASSERT(smem <= 200 * 1024, "QR panel too tall for the partition's shared-memory slices");
-      T* Ap = A.at(c0, c0);
-      i64 rs = A.rs, cs = A.cs;
-      int mpi = (int)mp, wi = (int)sw;
-      T* taus = H.at(s0, c0);
-      i64 tau_stride = H.rs + H.cs;
-      unsigned long long base = bar_count;
-      const T* ab = above2;
-      long long rows_below0 = (long long)(m - c0);
-      void* args[] = {&Ap, &rs, &cs, &mpi, &wi, &rows_per_cta, &taus, &tau_stride, &sc, &base, &ab, &rows_below0, &d_flag};
-      FB_CUDA_CHECK(cudaLaunchCooperativeKernel((void*)qr_panel_kernel<T>, dim3(G), dim3(QR_THREADS), args, smem, sp));
-      note_launch();
-      bar_count += (unsigned long long)std::min<i64>(sw, mp) * G;
-      View<const T> Vs = cview(A.sub(c0, c0, mp, sw));
-      View<T> Tss = H.sub(s0, c0, sw, sw);
-      householder_build_t<T>(sp, Vs, Tss);
-      const i64 rest = j0 + jb - (c0 + sw);
-      if (rest > 0) apply_block_householder_on_the_left<T>(sp, Vs, cview(Tss), A.sub(c0, c0 + sw, mp, rest), true, tmp_sp);
-    }
-    View<const T> Vb = cview(A.sub(j0, j0, m - j0, jb));
-    View<T> Tb = H.sub(0, j0, jb, jb);
-    if (jb > QR_PW) householder_build_t<T>(sp, Vb, Tb);
-    FB_CUDA_CHECK(cudaEventRecord(ev_block[(size_t)jblk], sp));
-  };
-  auto apply_block = [&](cudaStream_t s, i64 jblk, i64 c0, i64 c1, T* tmp) {  // block jblk's reflector on columns [c0, c1)
-    if (c1 <= c0) return;
-    const i64 j0 = jblk * bs, jb = std::min(bs, size - j0);
-    View<const T> Vb = cview(A.sub(j0, j0, m - j0, jb));
-    View<T> Tb = H.sub(0, j0, jb, jb);
-    apply_block_householder_on_the_left<T>(s, Vb, cview(Tb), A.sub(j0, c0, m - j0, c1 - c0), true, tmp);
-  };
-  factor_block(0);
-  for (i64 j = 0; j < nblk; ++j) {
-    const i64 c1 = std::min(size, (j + 1) * bs);               // first column right of block j
-    const i64 c2 = j + 1 < nblk ? std::min(size, (j + 2) * bs) : c1;  // end of block j + 1 (if any)
-    if (j + 1 < nblk) {
-      FB_CUDA_CHECK(cudaStreamWaitEvent(su, ev_block[(size_t)j], 0));
-      if (j >= 1) FB_CUDA_CHECK(cudaStreamWaitEvent(su, ev_first[(size_t)(j - 1)], 0));
-      apply_block(su, j, c1, c2, tmp_su);
-      FB_CUDA_CHECK(cudaEventRecord(ev_ready[(size_t)(j + 1)], su));
-      FB_CUDA_CHECK(cudaStreamWaitEvent(sp, ev_ready[(size_t)(j + 1)], 0));
-      factor_block(j + 1);
-    }
-    FB_CUDA_CHECK(cudaStreamWaitEvent(sm, ev_block[(size_t)j], 0));
-    if (c2 < n) {
-      const i64 c3 = j + 2 < nblk ? std::min(size, (j + 3) * bs) : c2;  // block j + 2 first: the next urgent one
-      if (c3 > c2) apply_block(sm, j, c2, c3, tmp_sm);
-      FB_CUDA_CHECK(cudaEventRecord(ev_first[(size_t)j], sm));
-      apply_block(sm, j, c3, n, tmp_sm);
-    } else {
-      FB_CUDA_CHECK(cudaEventRecord(ev_first[(size_t)j], sm));
-    }
-  }
-  int h_flag = 0;
-  FB_CUDA_CHECK(cudaMemcpyAsync(&h_flag, d_flag, sizeof(int), cudaMemcpyDeviceToHost, sp));
-  FB_CUDA_CHECK(cudaStreamSynchronize(sp));
-  FB_CUDA_CHECK(cudaStreamSynchronize(su));
-  FB_CUDA_CHECK(cudaStreamSynchronize(sm));
-  for (i64 j = 0; j < nblk; ++j) {
-    cudaEventDestroy(ev_block[(size_t)j]);
-    cudaEventDestroy(ev_ready[(size_t)j]);
-    cudaEventDestroy(ev_first[(size_t)j]);
-  }
-  cudaEventDestroy(ev_start);
-  ws_free(tmp_sm);
-  ws_free(tmp_su);
-  ws_free(tmp_sp);
-  ws_free(d_flag);
-  ws_free(scb);
-  return h_flag ? -1 : size;
-}
-
 // General driver: continues the factorization from the state (row, col) with the reference's column-skipping logic
 // (factor.rs:137-256 on sub-panels of <= QRG_PW columns; every sub-panel's reflector is applied to all the columns to its
 // right at once). `row` must be a multiple of the block size. Synchronous: one read-back per sub-panel. Returns the rank.
@@ -698,42 +563,12 @@ i64 qr_in_place(cudaStream_t st, View<T> A, View<T> H) {
   FB_ASSERT(bs > 0 && H.ncols == size, "Q_coeff must be block_size x min(nrows, ncols)");
   if (size == 0) return 0;
   FB_ASSERT(m < (1ll << 31) && n < (1ll << 31), "dimension too large");
-  if (const char* e = getenv("FAER_B200_QR_LOOKAHEAD")) {
-    // opt-in look-ahead driver (see above). The partition must hold the first (tallest) sub-panel's slices.
-    const int want = atoi(e);
-    const i64 need = (m * (i64)(QR_PW | 1) * (i64)sizeof(T) + 200 * 1024 - 1) / (200 * 1024);
-    cudaStream_t sp, su, sm;
-    int got = 0;
-    if (want > 0 && size >= 2 * bs && need <= 96) {
-      const int sms = (int)std::max<i64>(8, (std::max<i64>(need, want) + 7) / 8 * 8);
-      if (partition_streams(sms, &sp, &su, &sm, &got) && got > 0) {
-        const i64 g0 = std::min<i64>(std::min(got, 160), (m + 63) / 64);
-        const i64 rows0 = (m + g0 - 1) / g0;  // the first sub-panel is the tallest
-        if (rows0 * (i64)(QR_PW | 1) * (i64)sizeof(T) <= 200 * 1024) {
-          const i64 r = qr_in_place_lookahead<T>(st, A, H, sp, su, sm, got);
-          if (r >= 0) return r;
-          FB_ASSERT(false, "look-ahead QR driver met a rank-deficient column (use the default driver)");
-        }
-      }
-    }
-  }
   int dev = 0, num_sms = 0;
   FB_CUDA_CHECK(cudaGetDevice(&dev));
   FB_CUDA_CHECK(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev));
-  const int Gfull = std::min(num_sms, 160);  // the panel kernel's record reduction covers <= 160 CTAs
-  int Gmax = Gfull;
-  {
-    // fewer, fatter CTAs shorten the per-column grid exchange (barrier participants, records every CTA reads) at the price
-    // of longer per-CTA row loops; FAER_B200_QR_PANEL_CTAS caps the grid (the slices must still fit shared memory)
-    static int cap = -1;
-    if (cap < 0) {
-      const char* e = getenv("FAER_B200_QR_PANEL_CTAS");
-      cap = e ? atoi(e) : 0;
-    }
-    if (cap > 0) Gmax = std::min(Gmax, cap);
-  }
+  const int Gmax = std::min(num_sms, 160);  // the panel kernel's record reduction covers <= 160 CTAs
   // scratch
-  const size_t part_elems = (size_t)2 * Gfull * QR_NV, rowv_elems = (size_t)2 * QR_PW;
+  const size_t part_elems = (size_t)2 * Gmax * QR_NV, rowv_elems = (size_t)2 * QR_PW;
   char* scb = (char*)ws_alloc((part_elems + rowv_elems + QR_PW) * sizeof(T) + 64);
   QrScratch<T> sc;
   sc.part = (T*)scb;
@@ -773,11 +608,6 @@ i64 qr_in_place(cudaStream_t st, View<T> A, View<T> H) {
       }
       int G = (int)std::min<i64>(Gmax, (mp + 63) / 64);
       if (G < 1) G = 1;
-      {
-        // the slices must fit shared memory whatever the cap says
-        const i64 gmin = ((i64)mp * (i64)((int)sw | 1) * (i64)sizeof(T) + 200 * 1024 - 1) / (200 * 1024);
-        G = (int)std::min<i64>(std::max<i64>(G, gmin), std::min(num_sms, 160));
-      }
       int rows_per_cta = (int)((mp + G - 1) / G);
       const size_t smem = (size_t)rows_per_cta * (size_t)((int)sw | 1) * sizeof(T);
       FB_ASSERT(smem <= 200 * 1024, "QR panel too tall for the shared-memory slices");

@@ -28,28 +28,9 @@ cudaStream_t current_stream() { return g_stream; }
 void set_current_stream(cudaStream_t s) { g_stream = s; }
 
 namespace {
-struct StreamSms {
-  cudaStream_t st;
-  int sms;
-};
-std::vector<StreamSms> g_stream_sms;
 int g_device_sms = 0;
 }  // namespace
-void register_stream_sms(cudaStream_t st, int sms) {
-  std::lock_guard<std::mutex> lock(g_pool_mutex);
-  for (auto& e : g_stream_sms)
-    if (e.st == st) {
-      e.sms = sms;
-      return;
-    }
-  g_stream_sms.push_back(StreamSms{st, sms});
-}
-int stream_sms(cudaStream_t st) {
-  {
-    std::lock_guard<std::mutex> lock(g_pool_mutex);
-    for (auto& e : g_stream_sms)
-      if (e.st == st) return e.sms;
-  }
+int stream_sms(cudaStream_t) {
   if (g_device_sms == 0) {
     int dev = 0;
     FB_CUDA_CHECK(cudaGetDevice(&dev));

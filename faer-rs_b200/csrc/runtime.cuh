@@ -20,8 +20,6 @@ std::recursive_mutex& entry_mutex();
   std::lock_guard<std::recursive_mutex> fb_entry_lock_(::fb::entry_mutex()); \
   ::fb::require_device()
 bool is_device_pointer(const void* p);
-// SMs a stream may use: the device's count unless the stream belongs to a green-context partition (dist.cu registers
-// those). Persistent kernels size their grids with it.
 // Run-time options (C ABI: faer_b200_set_option / faer_b200_get_option; initial values from the environment):
 //   gemm_ws        FAER_B200_GEMM_WS        0 = never use the TMA / warp-specialised f64 GEMM, 1 = heuristic (default), 2 = always
 //                                           (128 x 64 tiles), 3 = always (128 x 128 tiles)
@@ -31,8 +29,9 @@ enum Option : int { OPT_GEMM_WS = 0, OPT_F64_GEMM_MODE = 1, OPT_COUNT };
 long long get_option(int opt);
 bool set_option_by_name(const char* name, long long value);
 long long get_option_by_name(const char* name);
+// SMs a kernel launched on `st` may use: the device's SM count (cached), for every stream, including those of dist.cu's
+// green-context partitions. Persistent kernels size their grids with it.
 int stream_sms(cudaStream_t st);
-void register_stream_sms(cudaStream_t st, int sms);
 
 // Optional per-launch timing of the dominant kernel (bench.py roofline): CUDA events around each GEMM launch.
 bool profiling_enabled();

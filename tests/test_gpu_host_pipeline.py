@@ -1,8 +1,9 @@
 """GPU tests of the host-pointer LLT path (block columns streamed through the factorization, dist.cu LltHostPipe).
 
-The default pipeline runs the same right-looking block-column driver on the same kernels as the device-resident path (so the
-factors are in fact bit-identical); the opt-in hybrid order (FAER_B200_HOST_LEFT=1: left-looking while the upload runs) groups
-the sums differently, hence the assertion is 1e-13 relative, not bitwise. On top of that the reference's contract is
+The pipeline runs the same right-looking block-column driver on the same kernels as the device-resident path, but in its first
+step each trailing block column is updated by its own launch once its upload has landed, where the device-resident path
+updates them all in one launch. The products are tiled differently and round differently in the last bit, hence the
+assertion is 1e-13 relative, not bitwise. On top of that the reference's contract is
 checked: the strict upper triangle of the host matrix is neither read nor written (cholesky/llt/factor.rs:68-97 reads the lower triangle only), and a non-positive pivot is reported with the
 same index (ldlt/factor.rs:146-150)."""
 import numpy as np
@@ -38,7 +39,7 @@ def test_host_llt_equals_device_llt(fb, cuda_dev, n):
     assert np.abs(A @ x - L @ (L.T @ x)).max() <= 1e-10 * np.abs(A).max() * n
 
 
-@pytest.mark.parametrize("bad", [1000, 3001])  # in the left-looking half / in the right-looking half
+@pytest.mark.parametrize("bad", [1000, 3001])  # an early and a later block column
 def test_host_llt_reports_the_failing_column(fb, bad):
     la = fb.linalg
     n = 4200

@@ -1,5 +1,6 @@
 """Dev aid: the LU panel chain in isolation — tall m x w panels through the recursive driver (non-square input => lu_rec on the
-current stream; FAER_B200_LU_CLUSTER=16 selects the cluster kernels incl. the fused sub-panel). usage: python tools/time_lu_panel.py [w ...]"""
+current stream, on the grid-barrier panel kernel: the cluster kernels and the fused sub-panel run only inside the
+partitioned look-ahead drivers). usage: python tools/time_lu_panel.py [w ...]"""
 import os
 import sys
 

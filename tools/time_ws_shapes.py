@@ -1,6 +1,6 @@
 """Dev aid: the ws f64 GEMM, narrow (gemm_ws = 2, 128 x 64 tiles) and wide (3, 128 x 128 tiles), against the cp.async kernel
 (0) on the trailing-update shapes of LLT / LU.
-usage: [FAER_B200_WS_STAGGER=0|1] python tools/time_ws_shapes.py"""
+usage: python tools/time_ws_shapes.py"""
 import os
 import sys
 
@@ -23,7 +23,6 @@ def best(f, reps=5):
     return b
 
 
-tag = f"stagger={os.environ.get('FAER_B200_WS_STAGGER', '1')}"
 # lower-triangular updates of the headline LLT (k = 512 / 256 / 128 by remaining order), and deeper ones; Add (accum 1)
 # is the LLT's, Replace (accum 0) skips the old-tile load
 for (n, k, accum) in [(16128, 128, 1), (16128, 256, 1), (16128, 512, 1), (16128, 768, 1), (16128, 1024, 1),
@@ -32,7 +31,7 @@ for (n, k, accum) in [(16128, 128, 1), (16128, 256, 1), (16128, 512, 1), (16128,
                       (3072, 128, 1)]:
     P = torch.randn((k, n), dtype=torch.float64, device=dev).T
     Cm = torch.randn((n, n), dtype=torch.float64, device=dev).T
-    line = f"{tag} SYRK(lower, {'Add' if accum else 'Replace'}) n={n} k={k}:"
+    line = f"SYRK(lower, {'Add' if accum else 'Replace'}) n={n} k={k}:"
     for mode in (0, 2, 3):
         lib.faer_b200_set_option(b"gemm_ws", mode)
         ms = best(lambda: la.matmul_triangular(Cm, 1, accum, P, 0, P.T, 0, -1.0))
@@ -45,7 +44,7 @@ for (m, n, k) in [(16384, 16384, 256), (16384, 16384, 512), (8192, 8192, 512), (
     L = torch.randn((k, m), dtype=torch.float64, device=dev).T
     U = torch.randn((n, k), dtype=torch.float64, device=dev).T
     Cm = torch.randn((n, m), dtype=torch.float64, device=dev).T
-    line = f"{tag} update m={m} n={n} k={k}:"
+    line = f"update m={m} n={n} k={k}:"
     for mode in (0, 2, 3):
         lib.faer_b200_set_option(b"gemm_ws", mode)
         ms = best(lambda: la.matmul(Cm, 1, L, U, -1.0))
