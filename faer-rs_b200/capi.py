@@ -623,6 +623,11 @@ def load() -> C.CDLL:
             "qr_reconstruct": ([MatMut, MatRef, MatRef, MatRef, P, MemAlloc], None),
             "qr_inverse_scratch": ([C.c_size_t, C.c_size_t, P], Layout),
             "qr_inverse": ([MatMut, MatRef, MatRef, MatRef, P, MemAlloc], None),
+            # include/faer_b200_fx128_svd.h
+            "BidiagParams": ([], BidiagParams),
+            "SvdParams": ([], SvdParams),
+            "svd_scratch": ([C.c_size_t, C.c_size_t, C.c_int, C.c_int, P, SvdParams], Layout),
+            "svd": ([MatRef, MatMut, VecMut, MatMut, P, MemAlloc, SvdParams], SvdStatus),
         }
         for name in ("solve_triangular_lower", "solve_triangular_upper", "solve_unit_triangular_lower",
                      "solve_unit_triangular_upper"):

@@ -511,7 +511,9 @@ int ed_num_levels(i64 n) {
   return lv;
 }
 
-// (d, e) scaled real tridiagonal on the device -> lam ascending, Z (n x n, ld n) its eigenvectors; false if a leaf failed
+}  // namespace
+
+// (d, e) real tridiagonal on the device -> lam ascending, Z (n x n, ld n) its eigenvectors; false if a leaf failed
 bool tridiag_dc_dd(cudaStream_t st, const dd* d_in, const dd* e_in, i64 n, dd* lam, dd* Z) {
   LaunchTag tag(LAUNCH_SOLVE);  // the merges' GEMMs included
   const int nlev = ed_num_levels(n);
@@ -603,6 +605,8 @@ bool tridiag_dc_dd(cudaStream_t st, const dd* d_in, const dd* e_in, i64 n, dd* l
   ws_free(pool);
   return h_fail == 0;
 }
+
+namespace {
 
 // ---- back-transform helpers ----
 // Uc (n x n, ld n) = D Z: Z's rows scaled by the phases (cx128) or copied (fx128)

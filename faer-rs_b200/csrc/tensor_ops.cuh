@@ -31,6 +31,14 @@ void householder_sequence_dd(cudaStream_t st, View<const dd> basis, View<const d
 // element units; false for non-finite input (evd_dd.cu)
 template <bool CX>
 bool self_adjoint_evd_dd(cudaStream_t st, View<const dd> A, View<dd> U, dd* S);
+// divide and conquer of the real symmetric tridiagonal (d, e) of order n (device arrays): lam ascending, Z (n x n, ld n) its
+// eigenvectors; false if a leaf did not converge (evd_dd.cu). Hidden, like svd_dd: the library exports only its C ABI additions.
+__attribute__((visibility("hidden"))) bool tridiag_dc_dd(cudaStream_t st, const dd* d, const dd* e, i64 n, dd* lam, dd* Z);
+// SVD (svd/mod.rs:530-672); U / V with ptr == nullptr or no columns: not computed (neither: values by bisection); U is
+// nrows x {size, nrows}, V is ncols x {size, ncols}; S: min(m, n) entries in element units, non-increasing; false for non-finite
+// input (svd_dd.cu)
+template <bool CX>
+__attribute__((visibility("hidden"))) bool svd_dd(cudaStream_t st, View<const dd> A, View<dd> U, dd* S, View<dd> V, double qr_ratio_threshold);
 
 inline void gemm(cudaStream_t st, VD dst, int ds, int accum, VCD lhs, int ls, VCD rhs, int rs, double alpha) {
   gemm_f64(st, dst, ds, accum, lhs, ls, rhs, rs, alpha);

@@ -727,5 +727,6 @@ void libfaer_v0_23_partial_piv_lu_solve_transpose_in_place_u64_c32(struct FaerV0
 #include "faer_b200_fx128.h"
 #include "faer_b200_fx128_qr.h"
 #include "faer_b200_fx128_evd.h"
+#include "faer_b200_fx128_svd.h"
 
 #endif /* LIBFAER_V0_24 */
