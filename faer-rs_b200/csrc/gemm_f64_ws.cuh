@@ -69,7 +69,10 @@ struct Shape {
   static constexpr int DST_BYTES = WIDE ? BM * BN * 8 : 0;  // 8 boxes of 16 rows x 128 columns, 128B-swizzled
   static constexpr int SMEM_BYTES = DST_BYTES + STAGES * STAGE_BYTES + 1024 /*alignment*/ + 128 /*barriers*/;
   // registers per thread after setmaxnreg; the launch gives every thread 65536 / THREADS (rounded down to a multiple of
-  // 8): 128 x 24 + 128 x 232 = 256 x 128, and 128 x 40 + 256 x 232 = 384 x 168
+  // 8): 128 x 24 + 128 x 232 = 256 x 128, and 128 x 40 + 256 x 232 = 384 x 168. ptxas allocates the consumer code at
+  // 232 (the 128 / 168 it reports is the launch value). Dropping the idle producer warps would not give the consumers
+  // more: each of the 4 SM sub-partitions has its own 16 K registers, and 10 warps per SM put 3 on some of them, which
+  // caps every thread at 168.
   static constexpr int PRODUCER_REGS = WIDE ? 40 : 24, CONSUMER_REGS = 232;
 };
 static_assert(Shape<true>::SMEM_BYTES <= 227 * 1024, "wide configuration exceeds the shared memory of one SM");
@@ -242,16 +245,15 @@ gemm_f64_ws_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
     // ================= producer warpgroup =================
     asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(S::PRODUCER_REGS));
     if (warp == 0 && lane == 0) {
-      uint32_t it = 0;  // global k-step counter: stage = it % STAGES, phase = (it / STAGES) & 1
-      uint32_t ds = 0;  // staged tiles so far
+      uint32_t s = 0, ph = 0;  // ring slot of the next k-step and the parity of its pass over the ring
+      uint32_t ds = 0;         // staged tiles so far
       for (int i = 0; i < p.tiles_per_cta; ++i) {
         int tm, tn;
         if (!walk.locate((int)blockIdx.x * p.tiles_per_cta + i, tm, tn)) break;
         const int m0 = tm * BM, n0 = tn * BN;
         const bool st = staged(tm, tn);
         const int dst_at = min(STAGES, nkt) - 1;
-        for (int kt = 0; kt < nkt; ++kt, ++it) {
-          const uint32_t s = it % STAGES, ph = (it / STAGES) & 1u;
+        for (int kt = 0; kt < nkt; ++kt) {
           mbar_wait(&empty[s], ph ^ 1u);
           const uint32_t sa = sstages + s * STAGE_BYTES, sb = sa + A_BYTES;
           mbar_expect_tx(&full[s], STAGE_BYTES);
@@ -280,6 +282,10 @@ gemm_f64_ws_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
               mbar_arrive(dst_full);
             }
             ++ds;
+          }
+          if (++s == STAGES) {
+            s = 0;
+            ph ^= 1u;
           }
         }
       }
@@ -314,9 +320,9 @@ gemm_f64_ws_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
   const int g = lane >> 2, t = lane & 3;
   const int wm0 = (cw & 3) * (WMI * 8), wn0 = (cw >> 2) * (WNI * 8);  // warp tile rows [wm0, wm0 + 32) x cols [wn0, wn0 + 64)
   // per-lane fragment offsets for the 4 k slots of a stage: k index K4(q, t) = {0,3,12,15}[t] ^ {0,1,4,5}[q]
+  const int base_k = (t == 0) ? 0 : (t == 1) ? 3 : (t == 2) ? 12 : 15;
   uint32_t offA[4][2], offB[4][2];  // [k slot][parity of the 8-row block] (MN-major) / [k slot][0] (K-major)
   {
-    const int base_k = (t == 0) ? 0 : (t == 1) ? 3 : (t == 2) ? 12 : 15;
 #pragma unroll
     for (int s = 0; s < 4; ++s) {
       const int kk = base_k ^ ((s & 1) | ((s & 2) << 1));
@@ -334,6 +340,11 @@ gemm_f64_ws_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
         offB[s][0] = off_mn_major(wn0 + g, kk);
         offB[s][1] = off_mn_major(wn0 + 8 + g, kk);
       }
+      // opaque to the compiler, so that it keeps the offsets in registers instead of rebuilding them from the thread
+      // index in every k-step (it does that when the register epilogue's accumulators and old values crowd them)
+      asm volatile("" : "+r"(offA[s][0]), "+r"(offB[s][0]));
+      if constexpr (!A_KMAJOR) asm volatile("" : "+r"(offA[s][1]));
+      if constexpr (!B_KMAJOR) asm volatile("" : "+r"(offB[s][1]));
     }
   }
 
@@ -348,8 +359,9 @@ gemm_f64_ws_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
     while (clock64() - t0 < p.stagger_cycles) __nanosleep(256);
   }
 
-  uint32_t it = 0;
-  uint32_t dc = 0;  // staged tiles so far
+  uint32_t s = 0, ph = 0;  // ring slot of the next k-step and the parity of its pass over the ring (as the producer's)
+  uint32_t sa = sstages;   // the slot's A tile; its B tile follows at + A_BYTES
+  uint32_t dc = 0;         // staged tiles so far
   for (int ti = 0; ti < p.tiles_per_cta; ++ti) {
     int tm, tn;
     if (!walk.locate((int)blockIdx.x * p.tiles_per_cta + ti, tm, tn)) break;
@@ -361,12 +373,10 @@ gemm_f64_ws_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
 #pragma unroll
       for (int j = 0; j < WNI; ++j) acc[i][j][0] = acc[i][j][1] = 0.0;
 
-    for (int kt = 0; kt < nkt; ++kt, ++it) {
-      const uint32_t s = it % STAGES, ph = (it / STAGES) & 1u;
+    for (int kt = 0; kt < nkt; ++kt) {
       double dk[4] = {1.0, 1.0, 1.0, 1.0};
       if constexpr (SPICY) {
         if (p.diag) {  // this lane's four k indices of the stage: K4(ss, t)
-          const int base_k = (t == 0) ? 0 : (t == 1) ? 3 : (t == 2) ? 12 : 15;
 #pragma unroll
           for (int ss = 0; ss < 4; ++ss) {
             const int kg = kt * BK + (base_k ^ ((ss & 1) | ((ss & 2) << 1)));
@@ -375,7 +385,7 @@ gemm_f64_ws_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
         }
       }
       mbar_wait(&full[s], ph);
-      const uint32_t sa = sstages + s * STAGE_BYTES, sb = sa + A_BYTES;
+      const uint32_t sb = sa + A_BYTES;
       // two DMMA.16x8x8 per 16 x 8 block and stage (the 16-deep shape's fragments do not fit beside the 128 accumulator
       // registers): half h contracts fragment k slots q = 2h + (v >> 1) (A) / 2h + i (B), i.e. stage indices K4(q, t).
       // A fragments of the whole warp tile, B fragments one 8-column block at a time.
@@ -408,6 +418,13 @@ gemm_f64_ws_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
       __syncwarp();
       if (lane == 0) mbar_arrive(&empty[s]);
+      if (++s == STAGES) {
+        s = 0;
+        ph ^= 1u;
+        sa = sstages;
+      } else {
+        sa += STAGE_BYTES;
+      }
     }
 
     if (staged(tm, tn)) {
@@ -458,7 +475,11 @@ gemm_f64_ws_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
       if (c_up && (row > col || (row == col && c_nodiag))) v = false;
       return v;
     };
-    double cv[2][WNI][2];
+    // wide: only the tiles on the diagonal of a triangular dst take this epilogue, so the old values of a row block are
+    // loaded just before it is combined. A second register set here would push the fragment offsets out of registers,
+    // and every k-step of every tile would reload them from local memory.
+    constexpr int CV = WIDE ? 1 : 2;
+    double cv[CV][WNI][2];
     auto load_old = [&](int i, double (&dst)[WNI][2]) {
       const int row = m0 + wm0 + i * 8 + g;
       const i64 roff = rowoff(row);
@@ -473,7 +494,11 @@ gemm_f64_ws_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
     if (add) load_old(0, cv[0]);
 #pragma unroll
     for (int i = 0; i < WMI; ++i) {
-      if (add && i + 1 < WMI) load_old(i + 1, cv[(i + 1) & 1]);
+      if constexpr (WIDE) {
+        if (add && i > 0) load_old(i, cv[0]);
+      } else {
+        if (add && i + 1 < WMI) load_old(i + 1, cv[(i + 1) & 1]);
+      }
       const int row = m0 + wm0 + i * 8 + g;
       const i64 roff = rowoff(row);
 #pragma unroll
@@ -481,7 +506,7 @@ gemm_f64_ws_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
           const int col = n0 + wn0 + j * 8 + 2 * t + e;
-          if (kept(row, col)) p.C[roff + coloff(col)] = add ? (alpha * acc[i][j][e] + cv[i & 1][j][e]) : alpha * acc[i][j][e];
+          if (kept(row, col)) p.C[roff + coloff(col)] = add ? (alpha * acc[i][j][e] + cv[i % CV][j][e]) : alpha * acc[i][j][e];
         }
       }
     }
