@@ -29,7 +29,6 @@
 // The algorithm is BLAS-2: each column reads and writes the trailing block once, so the kernel is HBM-bound.
 #include <algorithm>
 #include <climits>
-#include <type_traits>
 #include <vector>
 
 #include "ffi_common.cuh"
@@ -457,11 +456,6 @@ __global__ void cpq_tau_kernel(R* __restrict__ H, i64 rs, i64 cs, const R* __res
   }
 }
 
-inline void cpq_build_t(cudaStream_t st, View<const double> V, View<double> Tf, std::false_type) { householder_build_t<double>(st, V, Tf); }
-inline void cpq_build_t(cudaStream_t st, View<const float> V, View<float> Tf, std::false_type) { householder_build_t<float>(st, V, Tf); }
-inline void cpq_build_t(cudaStream_t st, View<const double> V, View<double> Tf, std::true_type) { householder_build_t_cx<double>(st, V, Tf); }
-inline void cpq_build_t(cudaStream_t st, View<const float> V, View<float> Tf, std::true_type) { householder_build_t_cx<float>(st, V, Tf); }
-
 }  // namespace
 
 // In-place column-pivoted QR (views in element units of the scalar kind; complex: COMPLEX units on an R* base). H: block_size x
@@ -469,7 +463,6 @@ inline void cpq_build_t(cudaStream_t st, View<const float> V, View<float> Tf, st
 // the column transpositions. Returns the transposition count.
 template <class R, bool CX>
 i64 colpiv_qr_in_place_t(cudaStream_t st, View<R> A, View<R> H, bool rs1, std::vector<long long>& trans) {
-  typedef std::integral_constant<bool, CX> Tag;
   constexpr int W = CX ? 2 : 1;
   const i64 m = A.nrows, n = A.ncols, size = std::min(m, n);
   FB_ASSERT(m < (i64)INT_MAX && n < (i64)INT_MAX, "column-pivoted QR: dimension too large");
@@ -529,7 +522,7 @@ i64 colpiv_qr_in_place_t(cudaStream_t st, View<R> A, View<R> H, bool rs1, std::v
     const i64 b = std::min(bs, size - j);
     View<const R> V{A.ptr + W * (j * A.rs + j * A.cs), m - j, b, A.rs, A.cs};
     View<R> Tf{H.ptr + W * (j * H.cs), b, b, H.rs, H.cs};
-    cpq_build_t(st, V, Tf, Tag());
+    householder_factor_t<R, CX>(st, V, Tf);
   }
 
   std::vector<int> hist((size_t)size);

@@ -379,22 +379,6 @@ void lu_rec_cx(cudaStream_t st, View<R> A, i64 start, i64 end, int* trans) {
   swap_cols(csub(A, 0, end, m, ncols - end));
 }
 
-// dst (compact column-major complex, ld = nrows) [i, c] = src[perm[i], c]
-template <class R>
-__global__ void gather_rows_cx_kernel(R* __restrict__ dst, const R* __restrict__ src, i64 rs, i64 cs, i64 nrows,
-                                       const long long* __restrict__ perm) {
-  const i64 i = (i64)blockIdx.x * blockDim.x + threadIdx.x;
-  const i64 c = blockIdx.y;
-  if (i < nrows) cst(dst, c * nrows + i, cld(src, perm[i] * rs + c * cs));
-}
-template <class R>
-__global__ void scatter_rows_cx_kernel(R* __restrict__ dst, i64 rs, i64 cs, const R* __restrict__ src, i64 nrows) {
-  const i64 i = (i64)blockIdx.x * blockDim.x + threadIdx.x;
-  const i64 c = blockIdx.y;
-  if (i < nrows) cst(dst, i * rs + c * cs, cld(src, c * nrows + i));
-}
-
-
 // conj?(T) X = rhs, T lower / upper triangular (unit diagonal or not); views in complex units
 template <class R>
 void solve_lower_triangular_in_place_cx(cudaStream_t st, View<const R> tril, bool unit, bool conj, View<R> rhs) {
@@ -434,14 +418,6 @@ LltResult llt_cholesky_in_place_cx(cudaStream_t st, View<R> A, R reg_delta, R re
   return res;
 }
 
-// L y = b, then L^H x = y (cholesky/llt/solve.rs:12-35 for complex L)
-template <class R>
-void llt_solve_in_place_cx(cudaStream_t st, View<const R> L, bool conj, View<R> rhs) {
-  FB_ASSERT(L.nrows == L.ncols && rhs.nrows == L.nrows, "LLT solve shape mismatch");
-  solve_lower_triangular_in_place_cx(st, L, false, conj, rhs);
-  solve_upper_triangular_in_place_cx(st, L.t(), false, !conj, rhs);
-}
-
 // In-place P A = L U of an m x n c64 matrix (views in complex units); perm arrays: HOST int64 of length m. Returns the
 // transposition count (lu_in_place, factor.rs:234-295).
 template <class R>
@@ -471,48 +447,6 @@ size_t lu_partial_piv_in_place_cx(cudaStream_t st, View<R> A, long long* perm_fw
   }
   for (i64 i = 0; i < m; ++i) perm_inv[perm_fwd[i]] = i;
   return n_trans;
-}
-
-// rhs[i, :] <- rhs[perm[i], :] (perm: HOST int64 of length nrows) through a compact copy
-template <class R>
-void permute_rows_cx(cudaStream_t st, View<R> rhs, const long long* perm) {
-  const i64 n = rhs.nrows, k = rhs.ncols;
-  if (n == 0 || k == 0) return;
-  FB_ASSERT(k < 65536, "too many right-hand sides for one permutation launch");
-  long long* d_perm = (long long*)ws_alloc((size_t)n * 8);
-  R* tmp = (R*)ws_alloc((size_t)n * (size_t)k * 2 * sizeof(R));
-  FB_CUDA_CHECK(cudaMemcpyAsync(d_perm, perm, (size_t)n * 8, cudaMemcpyHostToDevice, st));
-  dim3 grid((unsigned)((n + 255) / 256), (unsigned)k);
-  gather_rows_cx_kernel<R><<<grid, 256, 0, st>>>(tmp, rhs.ptr, rhs.rs, rhs.cs, n, d_perm);
-  scatter_rows_cx_kernel<R><<<grid, 256, 0, st>>>(rhs.ptr, rhs.rs, rhs.cs, tmp, n);
-  FB_CUDA_CHECK(cudaGetLastError());
-  note_launch();
-  note_launch();
-  FB_CUDA_CHECK(cudaStreamSynchronize(st));
-  ws_free(tmp);
-  ws_free(d_perm);
-}
-
-// rhs <- conj?(A)^-1 rhs from the factors (lu/partial_pivoting/solve.rs:21-54): permute rows, unit-lower solve, upper solve
-template <class R>
-void lu_solve_in_place_cx(cudaStream_t st, View<const R> L, View<const R> U, bool conj, const long long* perm_fwd, View<R> rhs) {
-  const i64 n = L.nrows;
-  FB_ASSERT(L.ncols == n && U.nrows == n && U.ncols == n && rhs.nrows == n, "LU solve shape mismatch");
-  if (n == 0 || rhs.ncols == 0) return;
-  permute_rows_cx<R>(st, rhs, perm_fwd);
-  solve_lower_triangular_in_place_cx(st, L, true, conj, rhs);
-  solve_upper_triangular_in_place_cx(st, U, false, conj, rhs);
-}
-
-// rhs <- conj?(A)^-T rhs (solve.rs:55-86): lower solve with U^T, unit-upper solve with L^T, then the inverse row permutation
-template <class R>
-void lu_solve_transpose_in_place_cx(cudaStream_t st, View<const R> L, View<const R> U, bool conj, const long long* perm_bwd, View<R> rhs) {
-  const i64 n = L.nrows;
-  FB_ASSERT(L.ncols == n && U.nrows == n && U.ncols == n && rhs.nrows == n, "LU solve shape mismatch");
-  if (n == 0 || rhs.ncols == 0) return;
-  solve_lower_triangular_in_place_cx(st, U.t(), false, conj, rhs);
-  solve_upper_triangular_in_place_cx(st, L.t(), true, conj, rhs);
-  permute_rows_cx<R>(st, rhs, perm_bwd);
 }
 
 // ---- Householder QR without pivoting for complex T: the unblocked leaf (qr/no_pivoting/factor.rs:11-86; householder.rs:59-107).
@@ -723,16 +657,8 @@ i64 qr_unblocked_t<float, true>(const QrCtx<float>& cx, View<float> A, View<floa
   LltResult llt_cholesky_in_place_##SUF(cudaStream_t st, View<R> A, R reg_delta, R reg_eps) {                                    \
     return llt_cholesky_in_place_cx<R>(st, A, reg_delta, reg_eps);                                                               \
   }                                                                                                                               \
-  void llt_solve_in_place_##SUF(cudaStream_t st, View<const R> L, bool conj, View<R> rhs) { llt_solve_in_place_cx<R>(st, L, conj, rhs); } \
   size_t lu_partial_piv_in_place_##SUF(cudaStream_t st, View<R> A, long long* perm_fwd, long long* perm_inv) {                   \
     return lu_partial_piv_in_place_cx<R>(st, A, perm_fwd, perm_inv);                                                             \
-  }                                                                                                                               \
-  void lu_solve_in_place_##SUF(cudaStream_t st, View<const R> L, View<const R> U, bool conj, const long long* perm_fwd, View<R> rhs) { \
-    lu_solve_in_place_cx<R>(st, L, U, conj, perm_fwd, rhs);                                                                      \
-  }                                                                                                                               \
-  void lu_solve_transpose_in_place_##SUF(cudaStream_t st, View<const R> L, View<const R> U, bool conj, const long long* perm_bwd, \
-                                         View<R> rhs) {                                                                           \
-    lu_solve_transpose_in_place_cx<R>(st, L, U, conj, perm_bwd, rhs);                                                            \
   }                                                                                                                               \
   i64 qr_in_place_##SUF(cudaStream_t st, View<R> A, View<R> Q_coeff, i64 blocking_threshold) {                                   \
     return qr_in_place_t<R, true>(st, A, Q_coeff, blocking_threshold);                                                           \

@@ -108,13 +108,12 @@ void ffi_cast(cudaStream_t st, TD* dst, i64 drs, i64 dcs, const TS* src, i64 srs
 // TMA-fed GEMM, SM partition) factor the widened matrix. The pivot search sees f64 values, so a pivot can differ from an all-f32
 // elimination's where two candidates agree to f32 precision (either choice is a valid partial pivot). The f32 solves run on the
 // native f32 triangular solves.
-size_t fb::lu_partial_piv_in_place_f32_via_f64(cudaStream_t st, VF A, void* perm_fwd, void* perm_bwd, int idx_bytes,
-                                               PartialPivLuParams params) {
+size_t fb::lu_partial_piv_in_place_f32_via_f64(cudaStream_t st, VF A, long long* perm_fwd, long long* perm_bwd) {
   const i64 m = A.nrows, n = A.ncols;
   const i64 ld = std::max<i64>(1, (m + 1) & ~(i64)1);
   double* W = (double*)ws_alloc((size_t)ld * (size_t)std::max<i64>(n, 1) * 8);
   ffi_cast<double, float>(st, W, 1, ld, A.ptr, A.rs, A.cs, m, n);
-  const size_t count = lu_partial_piv_in_place_f64(st, VD{W, m, n, 1, ld}, perm_fwd, perm_bwd, idx_bytes, params);
+  const size_t count = lu_partial_piv_in_place_f64(st, VD{W, m, n, 1, ld}, perm_fwd, perm_bwd);
   ffi_cast<float, double>(st, A.ptr, A.rs, A.cs, W, 1, ld, m, n);
   ws_free(W);
   return count;
@@ -122,8 +121,7 @@ size_t fb::lu_partial_piv_in_place_f32_via_f64(cudaStream_t st, VF A, void* perm
 
 extern "C" {
 
-// ---- the families every kind shares (ffi_entries.cuh); the reconstruct / inverse entries of f32 / c64 / c32 are in ffi_types.cu
-// except qr_reconstruct_f32, which runs on reconstruct.cu's real qr_reconstruct ----
+// ---- the families every kind shares (ffi_entries.cuh); the reconstruct / inverse entries of these kinds are in ffi_types.cu ----
 FB_MATMUL_FFI(f64, double, false)
 FB_MATMUL_FFI(f32, float, false)
 FB_MATMUL_FFI(c64, double, true)
@@ -144,11 +142,6 @@ FB_QR_FFI(f64, double, false)
 FB_QR_FFI(f32, float, false)
 FB_QR_FFI(c64, double, true)
 FB_QR_FFI(c32, float, true)
-FB_LLT_RECON_FFI(f64, double, false)
-FB_LU_RECON_FFI(f64, double, false)
-FB_QR_RECON_FFI(f64, double, false)
-FB_QR_RECON_FFI(f32, float, false)
-FB_QR_INV_FFI(f64, double, false)
 
 // ---- LDLT (no pivoting), f64: ldlt_f64.cu (the other dtypes, reconstruct and inverse: ffi_types.cu / ldlt_types.cu) ----
 FaerV0_24_LdltParams libfaer_v0_23_LdltParams_f64(void) {

@@ -5,10 +5,10 @@
 // function in the headers under include/): same argument order and meaning, by-value PODs, synchronous on return, abort() on
 // precondition violations. Host buffers are staged, device buffers are used in place, and `Par` / `MemAlloc` are ignored.
 //
-// Where a kind's driver is not the generic composition of tensor_ops.cuh, a body calls one per-kind hook (the `*_kind` functions).
-// The export macros at the end are instantiated by ffi.cu (f64, f32, c64, c32), ffi_types.cu (the triangular inverses and the
-// reconstruct / inverse entries it builds for the host too) and ffi_dd.cu (fx128, cx128). Scratch layouts are faer's formulas
-// with the kind's element size.
+// The solves, reconstructions and inverses are the compositions of tensor_ops.cuh / reconstruct_types.cu for every kind; only the
+// factorization drivers differ by kind (the `*_kind` functions). The export macros at the end are instantiated by ffi.cu (f64,
+// f32, c64, c32), ffi_types.cu (the triangular inverses and the reconstruct / inverse entries of the IEEE kinds, which it builds
+// for the host too) and ffi_dd.cu (fx128, cx128). Scratch layouts are faer's formulas with the kind's element size.
 #pragma once
 #include "ffi_common.cuh"
 #include "tensor_ops.cuh"
@@ -28,9 +28,8 @@ constexpr bool is_ieee_real_v = !CX && !is_dd_v<R>;
 
 // f32 partial-pivoting LU computed in f64 (ffi.cu): the matrix is widened on the device, factored by the f64 drivers and rounded
 // back. The factors carry one f32 rounding instead of an f32 elimination's accumulated ones. Hidden: the library exports the C ABI.
-__attribute__((visibility("hidden"))) size_t lu_partial_piv_in_place_f32_via_f64(cudaStream_t st, VF A, void* perm_fwd,
-                                                                                  void* perm_bwd, int idx_bytes,
-                                                                                  PartialPivLuParams params);
+__attribute__((visibility("hidden"))) size_t lu_partial_piv_in_place_f32_via_f64(cudaStream_t st, VF A, long long* perm_fwd,
+                                                                                  long long* perm_bwd);
 
 // The hooks and bodies below are static: each translation unit instantiates the ones it exports, and they are not exported
 // themselves. (Static rather than an anonymous namespace: nvcc's kernel stubs of a unit that also has a global anonymous namespace
@@ -44,58 +43,14 @@ static LltResult llt_kind(cudaStream_t st, View<R> A, R delta, R eps, FaerV0_24_
   else if constexpr (sizeof(R) == 8) return llt_cholesky_in_place_f64(st, A, delta, eps, LltParams{p.recursion_threshold, p.block_size});
   else return llt_cholesky_in_place_f32(st, A, delta, eps, LltParams{p.recursion_threshold, p.block_size});
 }
-// rhs <- conj?(L L^H)^-1 rhs (llt/solve.rs)
+// returns the transposition count; perm_fwd / perm_bwd: HOST int64 of A.nrows entries
 template <class R, bool CX>
-static void llt_solve_kind(cudaStream_t st, View<const R> L, bool conj, View<R> rhs) {
-  if constexpr (is_dd_v<R>) {
-    solve_lower_t<R, CX>(st, L, false, conj, rhs);
-    solve_upper_t<R, CX>(st, L.t(), false, CX && !conj, rhs);
-  } else if constexpr (CX && sizeof(R) == 8) llt_solve_in_place_c64(st, L, conj, rhs);
-  else if constexpr (CX) llt_solve_in_place_c32(st, L, conj, rhs);
-  else if constexpr (sizeof(R) == 8) llt_solve_in_place_f64(st, L, rhs);
-  else llt_solve_in_place_f32(st, L, rhs);
-}
-// returns the transposition count. The f64 driver (behind f32 too) writes the caller's permutations (host or device, u32 / u64)
-// itself; the other drivers return host permutations in pf / pb
-template <class R, bool CX>
-static size_t lu_kind(cudaStream_t st, View<R> A, void* perm_fwd, void* perm_bwd, int idx_bytes, FaerV0_24_PartialPivLuParams p,
-               std::vector<long long>& pf, std::vector<long long>& pb) {
-  if constexpr (is_ieee_real_v<R, CX>) {
-    const PartialPivLuParams params{p.recursion_threshold, p.block_size, p.par_threshold};
-    if constexpr (sizeof(R) == 8) return lu_partial_piv_in_place_f64(st, A, perm_fwd, perm_bwd, idx_bytes, params);
-    else return lu_partial_piv_in_place_f32_via_f64(st, A, perm_fwd, perm_bwd, idx_bytes, params);
-  } else {
-    pf.resize((size_t)A.nrows);
-    pb.resize((size_t)A.nrows);
-    if constexpr (is_dd_v<R>) return lu_dd<CX>(st, A, p.recursion_threshold, pf.data(), pb.data());
-    else if constexpr (sizeof(R) == 8) return lu_partial_piv_in_place_c64(st, A, pf.data(), pb.data());
-    else return lu_partial_piv_in_place_c32(st, A, pf.data(), pb.data());
-  }
-}
-// transpose = false: conj?(A)^-1 rhs with perm = perm_fwd (lu/partial_pivoting/solve.rs:21-54); true: conj?(A)^-T rhs with
-// perm = perm_bwd (solve.rs:55-86)
-template <class R, bool CX>
-static void lu_solve_kind(cudaStream_t st, View<const R> L, View<const R> U, bool conj, const long long* perm, View<R> rhs, bool transpose) {
-  if constexpr (is_f64_v<R, CX>) {
-    if (transpose) lu_solve_transpose_in_place_f64(st, L, U, perm, rhs);
-    else lu_solve_in_place_f64(st, L, U, perm, rhs);
-  } else if constexpr (CX && !is_dd_v<R>) {
-    if constexpr (sizeof(R) == 8) {
-      if (transpose) lu_solve_transpose_in_place_c64(st, L, U, conj, perm, rhs);
-      else lu_solve_in_place_c64(st, L, U, conj, perm, rhs);
-    } else {
-      if (transpose) lu_solve_transpose_in_place_c32(st, L, U, conj, perm, rhs);
-      else lu_solve_in_place_c32(st, L, U, conj, perm, rhs);
-    }
-  } else if (!transpose) {
-    permute_rows_t<R, CX>(st, rhs, perm);
-    solve_lower_t<R, CX>(st, L, true, conj, rhs);
-    solve_upper_t<R, CX>(st, U, false, conj, rhs);
-  } else {
-    solve_lower_t<R, CX>(st, U.t(), false, conj, rhs);
-    solve_upper_t<R, CX>(st, L.t(), true, conj, rhs);
-    permute_rows_t<R, CX>(st, rhs, perm);
-  }
+static size_t lu_kind(cudaStream_t st, View<R> A, FaerV0_24_PartialPivLuParams p, long long* perm_fwd, long long* perm_bwd) {
+  if constexpr (is_dd_v<R>) return lu_dd<CX>(st, A, p.recursion_threshold, perm_fwd, perm_bwd);
+  else if constexpr (CX && sizeof(R) == 8) return lu_partial_piv_in_place_c64(st, A, perm_fwd, perm_bwd);
+  else if constexpr (CX) return lu_partial_piv_in_place_c32(st, A, perm_fwd, perm_bwd);
+  else if constexpr (sizeof(R) == 8) return lu_partial_piv_in_place_f64(st, A, perm_fwd, perm_bwd);
+  else return lu_partial_piv_in_place_f32_via_f64(st, A, perm_fwd, perm_bwd);
 }
 // Householder QR without pivoting (qr/no_pivoting/factor.rs:258-301); returns the rank. The real IEEE drivers pick their own
 // blocking.
@@ -106,46 +61,6 @@ static i64 qr_kind(cudaStream_t st, View<R> A, View<R> Q, i64 blocking_threshold
   else if constexpr (sizeof(R) == 8) return qr_in_place_c64(st, A, Q, blocking_threshold);
   else return qr_in_place_c32(st, A, Q, blocking_threshold);
 }
-// rhs <- Q rhs (transpose = false) or Q^H rhs (true), Q conjugated under `conj` (householder.rs:724-808); real kinds ignore `conj`
-template <class R, bool CX>
-static void householder_kind(cudaStream_t st, View<const R> basis, View<const R> factor, bool conj, View<R> rhs, bool transpose) {
-  if constexpr (is_dd_v<R>) householder_sequence_dd<CX>(st, basis, factor, CX && conj, rhs, transpose);
-  else if constexpr (!CX) {
-    if (transpose) apply_block_householder_sequence_transpose_on_the_left<R>(st, basis, factor, rhs);
-    else apply_block_householder_sequence_on_the_left<R>(st, basis, factor, rhs);
-  } else if constexpr (sizeof(R) == 8) apply_householder_sequence_left_c64(st, basis, factor, conj, rhs, transpose);
-  else apply_householder_sequence_left_c32(st, basis, factor, conj, rhs, transpose);
-}
-// f64 reconstructs and inverts with reconstruct.cu's f64 functions, the other kinds with reconstruct_types.cu's compositions
-template <class R, bool CX>
-static void llt_recon_kind(cudaStream_t st, View<R> out, View<const R> L, bool inverse) {
-  if constexpr (is_f64_v<R, CX>) {
-    if (inverse) llt_inverse_f64(st, out, L);
-    else llt_reconstruct_f64(st, out, L);
-  } else {
-    if (inverse) llt_inverse_t<R, CX>(st, out, L);
-    else llt_reconstruct_t<R, CX>(st, out, L);
-  }
-}
-template <class R, bool CX>
-static void lu_recon_kind(cudaStream_t st, View<R> out, View<const R> L, View<const R> U, const long long* perm, bool inverse) {
-  if constexpr (is_f64_v<R, CX>) {
-    if (inverse) lu_inverse_f64(st, out, L, U, perm);
-    else lu_reconstruct_f64(st, out, L, U, perm);
-  } else {
-    if (inverse) lu_inverse_t<R, CX>(st, out, L, U, perm);
-    else lu_reconstruct_t<R, CX>(st, out, L, U, perm);
-  }
-}
-// the real IEEE kinds reconstruct with reconstruct.cu's qr_reconstruct; f64 inverts with its qr_inverse_f64
-template <class R, bool CX, bool INVERSE>
-static void qr_recon_kind(cudaStream_t st, View<R> out, View<const R> basis, View<const R> factor, View<const R> Rm) {
-  if constexpr (INVERSE && is_f64_v<R, CX>) qr_inverse_f64(st, out, basis, factor, Rm);
-  else if constexpr (INVERSE) qr_inverse_t<R, CX>(st, out, basis, factor, Rm);
-  else if constexpr (is_ieee_real_v<R, CX>) qr_reconstruct<R>(st, out, basis, factor, Rm);
-  else qr_reconstruct_t<R, CX>(st, out, basis, factor, Rm);
-}
-
 // The row permutation of the LU solves and reconstructions, of A.nrows entries (faer.hpp fills SliceRef.len with bytes, so `len`
 // is never used). An entry outside [0, n) aborts. fx128 / cx128 also abort on a null slice; the IEEE kinds do not test for it.
 template <class R>
@@ -229,7 +144,7 @@ static void llt_solve_entry(FaerV0_24_MatRef L, FaerV0_24_Conj A_conj, FaerV0_24
   FB_ASSERT(L.nrows == L.ncols && rhs.nrows == L.nrows, "LLT solve shape mismatch");
   cudaStream_t st = current_stream();
   StagedMat l = stage<R, CX>(L, st), r = stage<R, CX>(rhs, true, st);
-  llt_solve_kind<R, CX>(st, l.view<const R>(), CX && A_conj == FaerV0_24_Conj_Yes, r.view<R>());
+  llt_solve_t<R, CX>(st, l.view<const R>(), CX && A_conj == FaerV0_24_Conj_Yes, r.view<R>());
   finish_all(st, {&l, &r});
 }
 
@@ -242,8 +157,8 @@ static FaerV0_24_PartialPivLuStatus lu_factor_entry(FaerV0_24_MatMut A, FaerV0_2
   // is taken from A.nrows, never from `len`
   FB_ASSERT(A.nrows == 0 || (perm_fwd.ptr != nullptr && perm_bwd.ptr != nullptr), "null permutation slice");
   StagedMat a = stage<R, CX>(A, true, st);
-  std::vector<long long> pf, pb;
-  const size_t count = lu_kind<R, CX>(st, a.view<R>(), perm_fwd.ptr, perm_bwd.ptr, idx_bytes, params, pf, pb);
+  std::vector<long long> pf(A.nrows), pb(A.nrows);
+  const size_t count = lu_kind<R, CX>(st, a.view<R>(), params, pf.data(), pb.data());
   finish_all(st, {&a});
   write_perm(perm_fwd.ptr, pf, idx_bytes);
   write_perm(perm_bwd.ptr, pb, idx_bytes);
@@ -262,7 +177,7 @@ static void lu_solve_entry(FaerV0_24_MatRef L, FaerV0_24_MatRef U, FaerV0_24_Con
     if (n == 0 || rhs.ncols == 0) return;  // fx128 / cx128 stage nothing for an empty solve
   }
   StagedMat l = stage<R, CX>(L, st), u = stage<R, CX>(U, st), r = stage<R, CX>(rhs, true, st);
-  lu_solve_kind<R, CX>(st, l.view<const R>(), u.view<const R>(), CX && conj == FaerV0_24_Conj_Yes, p.data(), r.view<R>(), transpose);
+  lu_solve_t<R, CX>(st, l.view<const R>(), u.view<const R>(), CX && conj == FaerV0_24_Conj_Yes, p.data(), r.view<R>(), transpose);
   finish_all(st, {&l, &u, &r});
 }
 
@@ -284,7 +199,7 @@ static void householder_entry(FaerV0_24_MatRef basis, FaerV0_24_MatRef factor, F
   FB_ENTRY();
   cudaStream_t st = current_stream();
   StagedMat b = stage<R, CX>(basis, st), f = stage<R, CX>(factor, st), r = stage<R, CX>(rhs, true, st);
-  householder_kind<R, CX>(st, b.view<const R>(), f.view<const R>(), conj == FaerV0_24_Conj_Yes, r.view<R>(), transpose);
+  householder_sequence_t<R, CX>(st, b.view<const R>(), f.view<const R>(), conj == FaerV0_24_Conj_Yes, r.view<R>(), transpose);
   finish_all(st, {&b, &f, &r});
 }
 
@@ -312,9 +227,9 @@ static void qr_solve_entry(FaerV0_24_MatRef Qb, FaerV0_24_MatRef Qc, FaerV0_24_M
   const View<R> x = r.view<R>();
   if (mode == 2) {
     solve_lower_t<R, CX>(st, Rv.t(), false, cj, x);
-    householder_kind<R, CX>(st, b.view<const R>(), f.view<const R>(), !cj, x, false);  // conj composed with Yes
+    householder_sequence_t<R, CX>(st, b.view<const R>(), f.view<const R>(), !cj, x, false);  // conj composed with Yes
   } else {
-    householder_kind<R, CX>(st, b.view<const R>(), f.view<const R>(), !cj, x, true);
+    householder_sequence_t<R, CX>(st, b.view<const R>(), f.view<const R>(), !cj, x, true);
     solve_upper_t<R, CX>(st, Rv, false, cj, sub_t<R, CX>(x, 0, 0, (i64)size, x.ncols));
   }
   finish_all(st, {&b, &f, &r});
@@ -327,7 +242,8 @@ static void llt_recon_entry(FaerV0_24_MatMut A, FaerV0_24_MatRef L, bool inverse
   cudaStream_t st = current_stream();
   // only the lower triangle is written: the rest of A must survive the round trip
   StagedMat a = stage<R, CX>(A, true, st), l = stage<R, CX>(L, st);
-  llt_recon_kind<R, CX>(st, a.view<R>(), l.view<const R>(), inverse);
+  if (inverse) llt_inverse_t<R, CX>(st, a.view<R>(), l.view<const R>());
+  else llt_reconstruct_t<R, CX>(st, a.view<R>(), l.view<const R>());
   finish_all(st, {&a, &l});
 }
 
@@ -338,16 +254,18 @@ static void lu_recon_entry(FaerV0_24_MatMut A, FaerV0_24_MatRef L, FaerV0_24_Mat
   cudaStream_t st = current_stream();
   const std::vector<long long> p = read_lu_perm<R>(perm, L.nrows, idx_bytes);
   StagedMat a = stage<R, CX>(A, false, st), l = stage<R, CX>(L, st), u = stage<R, CX>(U, st);
-  lu_recon_kind<R, CX>(st, a.view<R>(), l.view<const R>(), u.view<const R>(), p.data(), inverse);
+  if (inverse) lu_inverse_t<R, CX>(st, a.view<R>(), l.view<const R>(), u.view<const R>(), p.data());
+  else lu_reconstruct_t<R, CX>(st, a.view<R>(), l.view<const R>(), u.view<const R>(), p.data());
   finish_all(st, {&a, &l, &u});
 }
 
-template <class R, bool CX, bool INVERSE>
-static void qr_recon_entry(FaerV0_24_MatMut A, FaerV0_24_MatRef Qb, FaerV0_24_MatRef Qc, FaerV0_24_MatRef Rm) {
+template <class R, bool CX>
+static void qr_recon_entry(FaerV0_24_MatMut A, FaerV0_24_MatRef Qb, FaerV0_24_MatRef Qc, FaerV0_24_MatRef Rm, bool inverse) {
   FB_ENTRY();
   cudaStream_t st = current_stream();
   StagedMat a = stage<R, CX>(A, false, st), b = stage<R, CX>(Qb, st), f = stage<R, CX>(Qc, st), r = stage<R, CX>(Rm, st);
-  qr_recon_kind<R, CX, INVERSE>(st, a.view<R>(), b.view<const R>(), f.view<const R>(), r.view<const R>());
+  if (inverse) qr_inverse_t<R, CX>(st, a.view<R>(), b.view<const R>(), f.view<const R>(), r.view<const R>());
+  else qr_reconstruct_t<R, CX>(st, a.view<R>(), b.view<const R>(), f.view<const R>(), r.view<const R>());
   finish_all(st, {&a, &b, &f, &r});
 }
 
@@ -617,7 +535,7 @@ static void qr_recon_entry(FaerV0_24_MatMut A, FaerV0_24_MatRef Qb, FaerV0_24_Ma
   void libfaer_v0_23_qr_reconstruct_##SUF(FaerV0_24_MatMut A, FaerV0_24_MatRef Q_basis, FaerV0_24_MatRef Q_coeff,               \
                                           FaerV0_24_MatRef R_, FaerV0_24_Par par, FaerV0_24_MemAlloc mem) {                     \
     (void)par; (void)mem;                                                                                                       \
-    fb::qr_recon_entry<R, CX, false>(A, Q_basis, Q_coeff, R_);                                                                  \
+    fb::qr_recon_entry<R, CX>(A, Q_basis, Q_coeff, R_, false);                                                                  \
   }
 #define FB_QR_INV_FFI(SUF, R, CX)                                                                                                \
   FaerV0_24_Layout libfaer_v0_23_qr_inverse_scratch_##SUF(size_t dim, size_t block_size, FaerV0_24_Par par) {                   \
@@ -627,5 +545,5 @@ static void qr_recon_entry(FaerV0_24_MatMut A, FaerV0_24_MatRef Qb, FaerV0_24_Ma
   void libfaer_v0_23_qr_inverse_##SUF(FaerV0_24_MatMut A, FaerV0_24_MatRef Q_basis, FaerV0_24_MatRef Q_coeff, FaerV0_24_MatRef R_, \
                                       FaerV0_24_Par par, FaerV0_24_MemAlloc mem) {                                              \
     (void)par; (void)mem;                                                                                                       \
-    fb::qr_recon_entry<R, CX, true>(A, Q_basis, Q_coeff, R_);                                                                   \
+    fb::qr_recon_entry<R, CX>(A, Q_basis, Q_coeff, R_, true);                                                                   \
   }

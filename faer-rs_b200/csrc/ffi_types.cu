@@ -1,5 +1,5 @@
 // extern "C" boundary, second translation unit: the entry points whose drivers are the flat-map files (reconstruct_types.cu,
-// ldlt_types.cu, cplx_condensed.cu) — `*_reconstruct` / `*_inverse` for f32 / c64 / c32 and the triangular inverses (both
+// ldlt_types.cu, cplx_condensed.cu) — `*_reconstruct` / `*_inverse` for f64 / f32 / c64 / c32 and the triangular inverses (both
 // instantiated from ffi_entries.cuh), LDLT beyond the f64 factorization, `svd` / `self_adjoint_evd` for complex T. Same conventions as ffi.cu (by-value PODs, synchronous on return, abort() on precondition
 // violations, host buffers staged, device buffers used in place). Kept apart from ffi.cu so that this unit, runtime.cu and the
 // three drivers also build for the host (tools/emul/ffi_types_host.cpp: the staging layer and the drivers end to end on the CPU).
@@ -291,16 +291,20 @@ FB_SVD_EVD_CPLX_FFI(c64, double)
 FB_SVD_EVD_CPLX_FFI(c32, float)
 #undef FB_SVD_EVD_CPLX_FFI
 
-// ---- reconstruct / inverse for f32 / c64 / c32 (ffi_entries.cuh; qr_reconstruct_f32 is in ffi.cu) and the triangular inverses of
-// every IEEE kind ----
+// ---- reconstruct / inverse (ffi_entries.cuh) and the triangular inverses of every IEEE kind ----
+FB_LLT_RECON_FFI(f64, double, false)
 FB_LLT_RECON_FFI(f32, float, false)
 FB_LLT_RECON_FFI(c64, double, true)
 FB_LLT_RECON_FFI(c32, float, true)
+FB_LU_RECON_FFI(f64, double, false)
 FB_LU_RECON_FFI(f32, float, false)
 FB_LU_RECON_FFI(c64, double, true)
 FB_LU_RECON_FFI(c32, float, true)
+FB_QR_RECON_FFI(f64, double, false)
+FB_QR_RECON_FFI(f32, float, false)
 FB_QR_RECON_FFI(c64, double, true)
 FB_QR_RECON_FFI(c32, float, true)
+FB_QR_INV_FFI(f64, double, false)
 FB_QR_INV_FFI(f32, float, false)
 FB_QR_INV_FFI(c64, double, true)
 FB_QR_INV_FFI(c32, float, true)

@@ -29,11 +29,8 @@ struct LltResult {
 void solve_lower_triangular_in_place_c64(cudaStream_t st, VCD tril, bool unit, bool conj, VD rhs);
 void solve_upper_triangular_in_place_c64(cudaStream_t st, VCD triu, bool unit, bool conj, VD rhs);
 LltResult llt_cholesky_in_place_c64(cudaStream_t st, VD A, double reg_delta, double reg_eps);
-void llt_solve_in_place_c64(cudaStream_t st, VCD L, bool conj, VD rhs);
-// c64 partial-pivoting LU (perm arrays: HOST int64 of length nrows) and the solve on its factors
+// c64 partial-pivoting LU (perm arrays: HOST int64 of length nrows)
 size_t lu_partial_piv_in_place_c64(cudaStream_t st, VD A, long long* perm_fwd, long long* perm_inv);
-void lu_solve_in_place_c64(cudaStream_t st, VCD L, VCD U, bool conj, const long long* perm_fwd, VD rhs);
-void lu_solve_transpose_in_place_c64(cudaStream_t st, VCD L, VCD U, bool conj, const long long* perm_bwd, VD rhs);
 // c64 Householder QR without pivoting (returns the rank) and rhs <- Q rhs / Q^H rhs by the block-Householder sequence
 i64 qr_in_place_c64(cudaStream_t st, VD A, VD Q_coeff, i64 blocking_threshold);
 void apply_householder_sequence_left_c64(cudaStream_t st, VCD basis, VCD factor, bool conj, VD rhs, bool transpose);
@@ -41,13 +38,6 @@ void apply_householder_sequence_left_c64(cudaStream_t st, VCD basis, VCD factor,
 // In-place lower Cholesky of the lower triangle of A (strict upper triangle untouched).
 // `reg_delta`/`reg_eps`: dynamic regularisation (active iff both > 0), reference llt/factor.rs:85-87.
 LltResult llt_cholesky_in_place_f64(cudaStream_t stream, VD A, double reg_delta, double reg_eps, LltParams params);
-
-// reconstruct.cu: `*_reconstruct` / `*_inverse` on the factors (f64); perm arrays are HOST int64
-void llt_reconstruct_f64(cudaStream_t st, VD out, VCD L);
-void llt_inverse_f64(cudaStream_t st, VD out, VCD L);
-void lu_reconstruct_f64(cudaStream_t st, VD out, VCD L, VCD U, const long long* perm_bwd_host);
-void lu_inverse_f64(cudaStream_t st, VD out, VCD L, VCD U, const long long* perm_fwd_host);
-void qr_inverse_f64(cudaStream_t st, VD out, VCD Q_basis, VCD Q_coeff, VCD R);
 
 // LDLT without pivoting (ldlt_f64.cu; reference cholesky/ldlt/factor.rs:725-767): D on the diagonal, unit-lower L strictly
 // below it, strict upper triangle untouched. d_signs: device int8[n] of expected pivot signs, or null.
@@ -65,22 +55,8 @@ void ldlt_solve_in_place_f64(cudaStream_t stream, VCD L, const double* D, i64 ds
 void llt_cholesky_device_f64(cudaStream_t stream, VD A, double reg_delta, double reg_eps, long long* d_info, i64 j0);
 
 // ---- lu::partial_pivoting::factor (reference: faer/src/linalg/lu/partial_pivoting/factor.rs:234-295) ----
-struct PartialPivLuParams {
-  size_t recursion_threshold;  // faer default 16
-  size_t block_size;           // faer default 64 (unused by the reference's recursive code)
-  size_t par_threshold;
-};
-// In-place P A = L U. perm_fwd / perm_inv: DEVICE arrays of nrows indices (u32 if idx_bytes==4 else u64).
-// Returns the transposition count.
-size_t lu_partial_piv_in_place_f64(cudaStream_t stream, VD A, void* perm_fwd, void* perm_inv, int idx_bytes,
-                                   PartialPivLuParams params);
-
-// ---- solves on top of the factors (solve_f64.cu; reference llt/solve.rs:12-35, lu/partial_pivoting/solve.rs:21-54) ----
-void permute_rows_in_place_f64(cudaStream_t stream, VD rhs, const long long* perm_fwd_host);
-void llt_solve_in_place_f64(cudaStream_t stream, VCD L, VD rhs);
-void lu_solve_in_place_f64(cudaStream_t stream, VCD L, VCD U, const long long* perm_fwd_host, VD rhs);
-// rhs <- A^-T rhs (lu/partial_pivoting/solve.rs:55-86); perm_bwd: HOST int64 array, the inverse row permutation
-void lu_solve_transpose_in_place_f64(cudaStream_t stream, VCD L, VCD U, const long long* perm_bwd_host, VD rhs);
+// In-place P A = L U. perm_fwd / perm_inv: HOST int64 arrays of nrows entries. Returns the transposition count.
+size_t lu_partial_piv_in_place_f64(cudaStream_t stream, VD A, long long* perm_fwd, long long* perm_inv);
 
 // workspace-based LU building blocks (used by dist.cu); all work is enqueued on the stream given at creation
 struct LuWorkspace;

@@ -1041,7 +1041,6 @@ struct LuCtx {
   int* plan_cnt;         // [ngroups_max]
   PanelScratch sc;
   unsigned long long bar_count;  // host mirror of the barrier counter
-  i64 recursion_threshold;       // reference's leaf width (<= it -> unblocked); GPU leaf = cooperative panel
   int cluster_ctas = 0;           // > 0: factor leaves with the cluster (DSMEM) panel kernel on this many CTAs
   cudaStream_t st_big = nullptr;  // optional: stream of a larger SM partition for the recursion's big TRSM / GEMM nodes
   cudaEvent_t ev_to_big = nullptr, ev_from_big = nullptr;
@@ -1264,13 +1263,10 @@ void lu_rec(LuCtx& ctx, VD A, i64 start, i64 end, int* trans) {
 
 }  // namespace
 
-size_t lu_partial_piv_in_place_f64(cudaStream_t stream, VD A, void* perm_fwd, void* perm_inv, int idx_bytes,
-                                   PartialPivLuParams params) {
+size_t lu_partial_piv_in_place_f64(cudaStream_t stream, VD A, long long* perm_fwd, long long* perm_inv) {
   const i64 m = A.nrows, n = A.ncols, size = std::min(m, n);
-  FB_ASSERT(idx_bytes == 4 || idx_bytes == 8, "index type must be u32 or u64");
   FB_ASSERT(m < (1ll << 31) && n < (1ll << 31), "dimension too large");
-  std::vector<long long> perm((size_t)m), pinv((size_t)m);
-  for (i64 i = 0; i < m; ++i) perm[(size_t)i] = i;
+  for (i64 i = 0; i < m; ++i) perm_fwd[i] = i;
   size_t n_trans = 0;
   // Large square column-major problems: right-looking block-column driver with two-stream look-ahead (dist.cu on a
   // single rank; same panel kernel => same pivots).
@@ -1278,14 +1274,13 @@ size_t lu_partial_piv_in_place_f64(cudaStream_t stream, VD A, void* perm_fwd, vo
   if (use_lookahead) {
     // block width: 512 up to n = 20000, 1024 beyond (FAER_B200_NB overrides)
     const i64 nbl = lookahead_block() ? lookahead_block() : (n <= 20000 ? 512 : 1024);
-    n_trans = dist_lu_f64(A.ptr, A.cs, n, nbl, perm.data(), pinv.data(), /*lookahead | local*/ 3);
+    n_trans = dist_lu_f64(A.ptr, A.cs, n, nbl, perm_fwd, perm_inv, /*lookahead | local*/ 3);
   } else if (size > 0) {
     LuCtx ctx;
     ctx.st = stream;
     int dev = 0;
     FB_CUDA_CHECK(cudaGetDevice(&dev));
     FB_CUDA_CHECK(cudaDeviceGetAttribute(&ctx.num_sms, cudaDevAttrMultiProcessorCount, dev));
-    ctx.recursion_threshold = (i64)params.recursion_threshold;
     const int G = ctx.num_sms;
     const i64 ngroups_max = (size + SWAP_GROUP - 1) / SWAP_GROUP + 1;
     ctx.d_trans = (int*)ws_alloc((size_t)size * sizeof(int));
@@ -1311,7 +1306,7 @@ size_t lu_partial_piv_in_place_f64(cudaStream_t stream, VD A, void* perm_fwd, vo
     for (i64 i = 0; i < size; ++i) {
       const int t = h_trans[(size_t)i];
       if (t != 0) {
-        std::swap(perm[(size_t)i], perm[(size_t)(i + t)]);
+        std::swap(perm_fwd[i], perm_fwd[i + t]);
         ++n_trans;
       }
     }
@@ -1326,29 +1321,7 @@ size_t lu_partial_piv_in_place_f64(cudaStream_t stream, VD A, void* perm_fwd, vo
     ws_free(ctx.plan_rows);
     ws_free(ctx.d_trans);
   }
-  for (i64 i = 0; i < m; ++i) pinv[(size_t)perm[(size_t)i]] = i;
-
-  // write the permutation arrays (host or device, u32 or u64)
-  auto put = [&](void* dst, const std::vector<long long>& v) {
-    if (m == 0) return;
-    std::vector<unsigned char> buf((size_t)m * idx_bytes);
-    for (i64 i = 0; i < m; ++i) {
-      if (idx_bytes == 4) ((uint32_t*)buf.data())[i] = (uint32_t)v[(size_t)i];
-      else ((uint64_t*)buf.data())[i] = (uint64_t)v[(size_t)i];
-    }
-    cudaPointerAttributes attr;
-    bool devp = false;
-    if (cudaPointerGetAttributes(&attr, dst) == cudaSuccess)
-      devp = attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged;
-    else
-      (void)cudaGetLastError();
-    if (devp)
-      FB_CUDA_CHECK(cudaMemcpy(dst, buf.data(), buf.size(), cudaMemcpyHostToDevice));
-    else
-      memcpy(dst, buf.data(), buf.size());
-  };
-  put(perm_fwd, perm);
-  put(perm_inv, pinv);
+  for (i64 i = 0; i < m; ++i) perm_inv[perm_fwd[i]] = i;
   return n_trans;
 }
 
@@ -1368,7 +1341,6 @@ LuWorkspace* lu_ws_create(cudaStream_t stream, i64 max_window, int sm_limit) {
   FB_CUDA_CHECK(cudaDeviceGetAttribute(&ctx.num_sms, cudaDevAttrMultiProcessorCount, dev));
   // a stream bound to an SM partition (green context): the cooperative panel grid must fit the partition
   if (sm_limit > 0 && sm_limit < ctx.num_sms) ctx.num_sms = sm_limit;
-  ctx.recursion_threshold = 16;
   const int G = ctx.num_sms;
   w->max_window = max_window;
   const i64 ngroups_max = (max_window + SWAP_GROUP - 1) / SWAP_GROUP + 1;

@@ -24,7 +24,6 @@
 // scan's verdict is read back before the loop, so that an indefinite input is returned untouched.
 #include <algorithm>
 #include <climits>
-#include <type_traits>
 #include <vector>
 
 #include "ffi_common.cuh"
@@ -390,22 +389,11 @@ __global__ void piv_copy_kernel(R* __restrict__ dst, i64 drs, i64 dcs, const R* 
   if (CX) p[1] = q[1];
 }
 
-// ---- the building blocks by scalar kind ----
-// L y = b, then L^H x = y, under A_conj (llt/solve.rs, the unpivoted solves)
-inline void piv_llt_solve(cudaStream_t st, VCD L, bool, VD rhs, std::false_type) { llt_solve_in_place_f64(st, L, rhs); }
-inline void piv_llt_solve(cudaStream_t st, VCF L, bool, VF rhs, std::false_type) { llt_solve_in_place_f32(st, L, rhs); }
-inline void piv_llt_solve(cudaStream_t st, VCD L, bool conj, VD rhs, std::true_type) { llt_solve_in_place_c64(st, L, conj, rhs); }
-inline void piv_llt_solve(cudaStream_t st, VCF L, bool conj, VF rhs, std::true_type) { llt_solve_in_place_c32(st, L, conj, rhs); }
 // tmp(lower) = L L^H (reconstruct) or L^-H L^-1 (inverse): the unpivoted compositions
 template <class R, bool CX>
 void piv_llt_product(cudaStream_t st, View<R> tmp, View<const R> L, bool inverse) {
   if (inverse) llt_inverse_t<R, CX>(st, tmp, L);
   else llt_reconstruct_t<R, CX>(st, tmp, L);
-}
-template <>
-void piv_llt_product<double, false>(cudaStream_t st, View<double> tmp, View<const double> L, bool inverse) {
-  if (inverse) llt_inverse_f64(st, tmp, L);
-  else llt_reconstruct_f64(st, tmp, L);
 }
 
 }  // namespace
@@ -539,7 +527,6 @@ PivLltResult piv_llt_in_place_t(cudaStream_t st, View<R> A, i64 block_size, std:
 // perm / perm_inv: host int64[n].
 template <class R, bool CX>
 void piv_llt_solve_t(cudaStream_t st, View<const R> L, const long long* perm, const long long* perm_inv, bool conj, View<R> rhs) {
-  typedef std::integral_constant<bool, CX> Tag;
   constexpr int W = CX ? 2 : 1;
   const i64 n = L.nrows, k = rhs.ncols;
   FB_ASSERT(L.ncols == n && rhs.nrows == n, "pivoted LLT solve shape mismatch");
@@ -550,7 +537,7 @@ void piv_llt_solve_t(cudaStream_t st, View<const R> L, const long long* perm, co
   FB_CUDA_CHECK(cudaMemcpyAsync(d_p + n, perm_inv, (size_t)n * 8, cudaMemcpyHostToDevice, st));
   View<R> X{tmp, n, k, 1, n};
   piv_gather_rows_t<R, CX>(st, X, View<const R>{rhs.ptr, n, k, rhs.rs, rhs.cs}, d_p);
-  piv_llt_solve(st, L, conj, X, Tag());
+  llt_solve_t<R, CX>(st, L, conj, X);
   piv_gather_rows_t<R, CX>(st, rhs, View<const R>{tmp, n, k, 1, n}, d_p + n);
   FB_CUDA_CHECK(cudaStreamSynchronize(st));  // the host permutations and the pool buffers are released below
   ws_free(tmp);

@@ -1,7 +1,6 @@
-// `*_reconstruct` / `*_inverse` on the factors for f32, c64 and c32 (SURVEY.md appendix C, "next" row; the f64 versions are in
-// reconstruct.cu and stay as they are). Same compositions as the f64 file, written once over the scalar kind <R, CX>
-// (R = real type, CX = interleaved complex): the structured product, the triangular solves, the LU solve, the row permutation
-// and the block-Householder sequence of that scalar kind — every one of them already on the hot path and validated on its own.
+// `*_reconstruct` / `*_inverse` on the factors for every scalar kind, written once over the scalar kind <R, CX> (R = real type,
+// CX = interleaved complex): the structured product, the triangular solves, the LU solve, the row permutation and the
+// block-Householder sequence of that scalar kind — every one of them already on the hot path and validated on its own.
 // Complex views are in COMPLEX element units on an R* base (the convention of gemm_c64 / cplx.cu).
 // Reference:
 //   cholesky/llt/reconstruct.rs:12-33   out(lower) = L(lower) * L^H(upper)            (only the lower triangle is written)
@@ -10,7 +9,7 @@
 //   lu/partial_pivoting/inverse.rs:11-49       A^-1 from the factors; here as the LU solve applied to the identity
 //   qr/no_pivoting/reconstruct.rs:13-39 out = [R; 0], then out <- Q out (sequence on the left, Conj::No)
 //   qr/no_pivoting/inverse.rs:11-43     A^-1 = R^-1 Q^H; here as the QR solve applied to the identity (Q^H first, then R^-1)
-// Tests: tests/test_gpu_zzzzzzzzz_2_reconstruct_types.py.
+// Tests: tests/test_gpu_zz4_reconstruct_inverse.py (f64), tests/test_gpu_zzzzzzzzz_2_reconstruct_types.py.
 #include <algorithm>
 
 #if defined(__CUDACC__)
@@ -105,47 +104,12 @@ struct RtCopyTriangle {
   }
 };
 
+// A <- the n x n identity
 template <class R, bool CX>
-struct Kind {
-  static constexpr int W = CX ? 2 : 1;
-  typedef View<R> V;
-  typedef View<const R> VC;
-
-  static void set_identity(cudaStream_t st, V A) {
-    const i64 n = A.nrows;
-    DevRun run{st};
-    run(RtSetIdentity<R, W>{A.ptr, A.rs, A.cs, n}, n, n);
-  }
-  // rhs[i, :] <- rhs[perm[i], :]; perm: HOST int64 of rhs.nrows entries
-  static void permute_rows(cudaStream_t st, V rhs, const long long* perm) {
-    const i64 n = rhs.nrows, k = rhs.ncols;
-    if (n == 0 || k == 0) return;
-    long long* d_perm = (long long*)ws_alloc((size_t)n * 8);
-    R* tmp = (R*)ws_alloc((size_t)n * (size_t)k * W * sizeof(R));
-    FB_CUDA_CHECK(cudaMemcpyAsync(d_perm, perm, (size_t)n * 8, cudaMemcpyHostToDevice, st));
-    DevRun run{st};
-    run(RtGatherRows<R, W>{tmp, rhs.ptr, rhs.rs, rhs.cs, n, k, d_perm}, n, k);
-    run(RtScatterBack<R, W>{rhs.ptr, rhs.rs, rhs.cs, tmp, n, k}, n, k);
-    FB_CUDA_CHECK(cudaStreamSynchronize(st));  // perm (host, pageable) and the pool buffers are released below
-    ws_free(tmp);
-    ws_free(d_perm);
-  }
-};
-
-// rhs <- Q rhs (adjoint = false) or Q^H rhs (adjoint = true); Q^H is the transposed sequence with Conj::Yes composed in
-// (householder.rs:768-808 as qr/no_pivoting/solve.rs:60-67 calls it)
-template <class R, bool CX>
-void rt_hh_seq(cudaStream_t st, View<const R> b, View<const R> f, View<R> rhs, bool adjoint) {
-  if constexpr (std::is_same_v<R, dd>) {
-    householder_sequence_dd<CX>(st, b, f, adjoint, rhs, adjoint);
-  } else if constexpr (!CX) {
-    if (adjoint) apply_block_householder_sequence_transpose_on_the_left<R>(st, b, f, rhs);
-    else apply_block_householder_sequence_on_the_left<R>(st, b, f, rhs);
-  } else if constexpr (sizeof(R) == 8) {
-    apply_householder_sequence_left_c64(st, b, f, adjoint, rhs, adjoint);
-  } else {
-    apply_householder_sequence_left_c32(st, b, f, adjoint, rhs, adjoint);
-  }
+void set_identity(cudaStream_t st, View<R> A) {
+  const i64 n = A.nrows;
+  DevRun run{st};
+  run(RtSetIdentity<R, CX ? 2 : 1>{A.ptr, A.rs, A.cs, n}, n, n);
 }
 
 }  // namespace
@@ -160,13 +124,13 @@ void llt_reconstruct_t(cudaStream_t st, View<R> out, View<const R> L) {
 
 template <class R, bool CX>
 void llt_inverse_t(cudaStream_t st, View<R> out, View<const R> L) {
-  typedef Kind<R, CX> K;
   const i64 n = out.nrows;
   FB_ASSERT(out.ncols == n && L.nrows == n && L.ncols == n, "llt_inverse shape mismatch");
   if (n == 0) return;
-  R* buf = (R*)ws_alloc((size_t)n * (size_t)n * K::W * sizeof(R));
+  constexpr int W = CX ? 2 : 1;
+  R* buf = (R*)ws_alloc((size_t)n * (size_t)n * W * sizeof(R));
   View<R> Li{buf, n, n, 1, n};
-  K::set_identity(st, Li);
+  set_identity<R, CX>(st, Li);
   solve_lower_t<R, CX>(st, L, false, false, Li);  // L_inv: lower triangular, exact zeros above the diagonal
   gemm_t<R, CX>(st, out, TRI_LOWER, 0, cview(Li).t(), TRI_UPPER, true, cview(Li), TRI_LOWER, false, R(1));  // adjoint(L_inv) * L_inv
   FB_CUDA_CHECK(cudaStreamSynchronize(st));
@@ -176,7 +140,6 @@ void llt_inverse_t(cudaStream_t st, View<R> out, View<const R> L) {
 // perm_bwd: HOST int64[m], the inverse row permutation
 template <class R, bool CX>
 void lu_reconstruct_t(cudaStream_t st, View<R> out, View<const R> L, View<const R> U, const long long* perm_bwd) {
-  typedef Kind<R, CX> K;
   const i64 m = L.nrows, n = U.ncols, size = std::min(m, n);
   FB_ASSERT(out.nrows == m && out.ncols == n && L.ncols >= size && U.nrows >= size, "lu_reconstruct shape mismatch");
   if (m == 0 || n == 0) return;
@@ -189,43 +152,37 @@ void lu_reconstruct_t(cudaStream_t st, View<R> out, View<const R> L, View<const 
     gemm_t<R, CX>(st, sub_t<R, CX>(out, 0, size, size, n - size), RECT, 0, Ls, UNIT_LOWER, false, sub_t<R, CX>(U, 0, size, size, n - size),
                   RECT, false, R(1));
   // (P A)[i, :] = A[perm_fwd[i], :]  =>  A[j, :] = (L U)[perm_bwd[j], :]
-  K::permute_rows(st, out, perm_bwd);
+  permute_rows_t<R, CX>(st, out, perm_bwd);
 }
 
 template <class R, bool CX>
 void lu_inverse_t(cudaStream_t st, View<R> out, View<const R> L, View<const R> U, const long long* perm_fwd) {
-  typedef Kind<R, CX> K;
   const i64 n = out.nrows;
   FB_ASSERT(out.ncols == n && L.nrows == n && L.ncols == n && U.nrows == n && U.ncols == n, "lu_inverse shape mismatch");
   if (n == 0) return;
-  // lu/partial_pivoting/solve.rs:21-54 on the identity: rows permuted, unit-lower solve, upper solve
-  K::set_identity(st, out);
-  K::permute_rows(st, out, perm_fwd);
-  solve_lower_t<R, CX>(st, L, true, false, out);
-  solve_upper_t<R, CX>(st, U, false, false, out);
+  set_identity<R, CX>(st, out);
+  lu_solve_t<R, CX>(st, L, U, false, perm_fwd, out, false);
 }
 
 template <class R, bool CX>
 void qr_reconstruct_t(cudaStream_t st, View<R> out, View<const R> Qb, View<const R> Qc, View<const R> Rm) {
-  typedef Kind<R, CX> K;
   const i64 m = Qb.nrows, n = Rm.ncols, size = std::min(m, n);
   FB_ASSERT(out.nrows == m && out.ncols == n && Qb.ncols == size && Qc.nrows > 0 && Qc.ncols == size && Rm.nrows == size,
             "qr_reconstruct shape mismatch");
   if (m == 0 || n == 0) return;
   DevRun run{st};
-  run(RtSetUpperTrapezoid<R, K::W>{out.ptr, out.rs, out.cs, m, n, Rm.ptr, Rm.rs, Rm.cs, size}, m, n);
-  if (size > 0) rt_hh_seq<R, CX>(st, Qb, Qc, out, false);
+  run(RtSetUpperTrapezoid<R, CX ? 2 : 1>{out.ptr, out.rs, out.cs, m, n, Rm.ptr, Rm.rs, Rm.cs, size}, m, n);
+  if (size > 0) householder_sequence_t<R, CX>(st, Qb, Qc, false, out, false);
 }
 
 template <class R, bool CX>
 void qr_inverse_t(cudaStream_t st, View<R> out, View<const R> Qb, View<const R> Qc, View<const R> Rm) {
-  typedef Kind<R, CX> K;
   const i64 n = out.nrows;
   FB_ASSERT(out.ncols == n && Qb.nrows == n && Qb.ncols == n && Qc.nrows > 0 && Qc.ncols == n && Rm.nrows == n && Rm.ncols == n,
             "qr_inverse shape mismatch");
   if (n == 0) return;
-  K::set_identity(st, out);
-  rt_hh_seq<R, CX>(st, Qb, Qc, out, true);          // Q^H
+  set_identity<R, CX>(st, out);
+  householder_sequence_t<R, CX>(st, Qb, Qc, true, out, true);  // Q^H
   solve_upper_t<R, CX>(st, Rm, false, false, out);  // R^-1 Q^H
 }
 
@@ -233,17 +190,17 @@ void qr_inverse_t(cudaStream_t st, View<R> out, View<const R> Qb, View<const R> 
 // only the triangle is written (the diagonal too unless `unit`). Here as the triangular solve applied to the identity.
 template <class R, bool CX>
 void inverse_triangular_t(cudaStream_t st, View<R> dst, View<const R> src, bool lower, bool unit) {
-  typedef Kind<R, CX> K;
   const i64 n = dst.nrows;
   FB_ASSERT(dst.ncols == n && src.nrows == n && src.ncols == n, "inverse_triangular shape mismatch");
   if (n == 0) return;
-  R* buf = (R*)ws_alloc((size_t)n * (size_t)n * K::W * sizeof(R));
+  constexpr int W = CX ? 2 : 1;
+  R* buf = (R*)ws_alloc((size_t)n * (size_t)n * W * sizeof(R));
   View<R> X{buf, n, n, 1, n};
-  K::set_identity(st, X);
+  set_identity<R, CX>(st, X);
   if (lower) solve_lower_t<R, CX>(st, src, unit, false, X);
   else solve_upper_t<R, CX>(st, src, unit, false, X);
   DevRun run{st};
-  run(RtCopyTriangle<R, K::W>{dst.ptr, dst.rs, dst.cs, buf, 1, n, n, lower ? 1 : 0, unit ? 1 : 0}, n, n);
+  run(RtCopyTriangle<R, W>{dst.ptr, dst.rs, dst.cs, buf, 1, n, n, lower ? 1 : 0, unit ? 1 : 0}, n, n);
   FB_CUDA_CHECK(cudaStreamSynchronize(st));
   ws_free(buf);
 }
@@ -263,6 +220,7 @@ template void inverse_triangular_t<dd, true>(cudaStream_t, View<dd>, View<const 
   template void lu_inverse_t<R, CX>(cudaStream_t, View<R>, View<const R>, View<const R>, const long long*);                      \
   template void qr_reconstruct_t<R, CX>(cudaStream_t, View<R>, View<const R>, View<const R>, View<const R>);                     \
   template void qr_inverse_t<R, CX>(cudaStream_t, View<R>, View<const R>, View<const R>, View<const R>);
+FB_RECON_INST(double, false)
 FB_RECON_INST(float, false)
 FB_RECON_INST(double, true)
 FB_RECON_INST(float, true)
@@ -282,7 +240,18 @@ FB_RECON_INST_DD(true)
 
 template <class R, bool CX>
 void permute_rows_t(cudaStream_t st, View<R> rhs, const long long* perm) {
-  Kind<R, CX>::permute_rows(st, rhs, perm);
+  constexpr int W = CX ? 2 : 1;
+  const i64 n = rhs.nrows, k = rhs.ncols;
+  if (n == 0 || k == 0) return;
+  long long* d_perm = (long long*)ws_alloc((size_t)n * 8);
+  R* tmp = (R*)ws_alloc((size_t)n * (size_t)k * W * sizeof(R));
+  FB_CUDA_CHECK(cudaMemcpyAsync(d_perm, perm, (size_t)n * 8, cudaMemcpyHostToDevice, st));
+  DevRun run{st};
+  run(RtGatherRows<R, W>{tmp, rhs.ptr, rhs.rs, rhs.cs, n, k, d_perm}, n, k);
+  run(RtScatterBack<R, W>{rhs.ptr, rhs.rs, rhs.cs, tmp, n, k}, n, k);
+  FB_CUDA_CHECK(cudaStreamSynchronize(st));  // perm (host, pageable) and the pool buffers are released below
+  ws_free(tmp);
+  ws_free(d_perm);
 }
 template void permute_rows_t<double, false>(cudaStream_t, View<double>, const long long*);
 template void permute_rows_t<float, false>(cudaStream_t, View<float>, const long long*);

@@ -327,8 +327,7 @@ bool evd_general(cudaStream_t st, View<const TO> A, View<TO> UL, View<TO> UR, TO
       note_launch();
       const VCD basis{(const double*)(H + 1), n - 1, n - 1, 1, n}, factor{(const double*)Hf, bs, n - 1, 1, bs};
       const VD z11{(double*)(Z + 1 + n), n - 1, n - 1, 1, n};
-      if (CX) apply_householder_sequence_left_c64(st, basis, factor, false, z11, false);
-      else apply_block_householder_sequence_on_the_left<double>(st, basis, factor, z11);
+      householder_sequence_t<double, CX>(st, basis, factor, false, z11, false);
     }
     hessenberg_part_kernel<S><<<grid2d(n), 256, 0, st>>>(H, nullptr, n);
     note_launch();

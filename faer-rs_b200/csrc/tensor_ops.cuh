@@ -105,6 +105,52 @@ void apply_block_householder_sequence_on_the_left(cudaStream_t st, View<const T>
 template <class T>
 void apply_block_householder_sequence_transpose_on_the_left(cudaStream_t st, View<const T> basis, View<const T> factor,
                                                             View<T> M);
+// cplx.cu: T(strict upper) <- V^H V for complex reflectors (upgrade_householder_factor with prev_block_size 1; views in COMPLEX
+// element units on an R* base), the twin of householder_build_t
+template <class R>
+void householder_build_t_cx(cudaStream_t st, View<const R> V, View<R> Tf);
+// rhs[i, :] <- rhs[perm[i], :] for every scalar kind (perm: HOST int64 of rhs.nrows entries; reconstruct_types.cu); a column
+// permutation is this on the transposed view
+template <class R, bool CX>
+void permute_rows_t(cudaStream_t st, View<R> rhs, const long long* perm);
+
+// ---- the compositions on the factors, over the scalar kind <R, CX> ----
+// rhs <- conj?(L L^H)^-1 rhs (llt/solve.rs:12-35): L y = rhs, then L^H x = y
+template <class R, bool CX>
+inline void llt_solve_t(cudaStream_t st, View<const R> L, bool conj, View<R> rhs) {
+  solve_lower_t<R, CX>(st, L, false, conj, rhs);
+  solve_upper_t<R, CX>(st, L.t(), false, CX && !conj, rhs);
+}
+// transpose = false: rhs <- conj?(A)^-1 rhs with perm = perm_fwd (lu/partial_pivoting/solve.rs:21-54); true: conj?(A)^-T rhs with
+// perm = perm_bwd (solve.rs:55-86). perm: HOST int64 of rhs.nrows entries
+template <class R, bool CX>
+inline void lu_solve_t(cudaStream_t st, View<const R> L, View<const R> U, bool conj, const long long* perm, View<R> rhs, bool transpose) {
+  if (!transpose) {
+    permute_rows_t<R, CX>(st, rhs, perm);
+    solve_lower_t<R, CX>(st, L, true, conj, rhs);
+    solve_upper_t<R, CX>(st, U, false, conj, rhs);
+  } else {
+    solve_lower_t<R, CX>(st, U.t(), false, conj, rhs);
+    solve_upper_t<R, CX>(st, L.t(), true, conj, rhs);
+    permute_rows_t<R, CX>(st, rhs, perm);
+  }
+}
+// rhs <- Q rhs (transpose = false) or Q^H rhs (true), Q conjugated under `conj` (householder.rs:724-808); real kinds ignore `conj`
+template <class R, bool CX>
+inline void householder_sequence_t(cudaStream_t st, View<const R> basis, View<const R> factor, bool conj, View<R> rhs, bool transpose) {
+  if constexpr (std::is_same_v<R, dd>) householder_sequence_dd<CX>(st, basis, factor, CX && conj, rhs, transpose);
+  else if constexpr (!CX) {
+    if (transpose) apply_block_householder_sequence_transpose_on_the_left<R>(st, basis, factor, rhs);
+    else apply_block_householder_sequence_on_the_left<R>(st, basis, factor, rhs);
+  } else if constexpr (sizeof(R) == 8) apply_householder_sequence_left_c64(st, basis, factor, conj, rhs, transpose);
+  else apply_householder_sequence_left_c32(st, basis, factor, conj, rhs, transpose);
+}
+// T(strict upper) <- V^H V for the reflectors stored in V, for the IEEE kinds
+template <class R, bool CX>
+inline void householder_factor_t(cudaStream_t st, View<const R> V, View<R> Tf) {
+  if constexpr (CX) householder_build_t_cx<R>(st, V, Tf);
+  else householder_build_t<R>(st, V, Tf);
+}
 
 // ---- qr.cu ----
 // Householder QR without pivoting, reference qr/no_pivoting/factor.rs:258-301. H: block_size x min(m, n).
@@ -117,10 +163,6 @@ i64 qr_recommended_block_size(i64 nrows, i64 ncols);
 // A = U B V^H, m >= n, column-major A. Reference: svd/bidiag.rs:47-256. Hl: bl x n, Hr: br x (n-1) (T blocks).
 template <class T>
 void bidiag_in_place(cudaStream_t st, View<T> A, View<T> Hl, View<T> Hr);
-// ---- reconstruct.cu ----
-// out = Q [R; 0]  (qr/no_pivoting/reconstruct.rs:13-39)
-template <class T>
-void qr_reconstruct(cudaStream_t st, View<T> out, View<const T> Q_basis, View<const T> Q_coeff, View<const T> R);
 // ---- evd.cu ----
 // S (device, compact, n entries) <- eigenvalues (nondecreasing) of the self-adjoint matrix whose lower triangle is in A
 // (evd/mod.rs:270-353 with u = None)
@@ -173,8 +215,8 @@ bool tridiag_dc_f64(cudaStream_t st, const double* d, const double* e, i64 n, do
 template <class T>
 void tridiag_in_place(cudaStream_t st, View<T> A, View<T> H);
 
-// ---- reconstruct_types.cu: `*_reconstruct` / `*_inverse` on the factors for the scalar kinds <float, false> (f32),
-// <double, true> (c64), <float, true> (c32); complex views in COMPLEX element units on an R* base; perm arrays HOST int64 ----
+// ---- reconstruct_types.cu: `*_reconstruct` / `*_inverse` on the factors for every scalar kind; complex views in COMPLEX element
+// units on an R* base; perm arrays HOST int64 ----
 template <class R, bool CX>
 void llt_reconstruct_t(cudaStream_t st, View<R> out, View<const R> L);
 template <class R, bool CX>
@@ -188,18 +230,10 @@ void qr_reconstruct_t(cudaStream_t st, View<R> out, View<const R> Q_basis, View<
 template <class R, bool CX>
 void qr_inverse_t(cudaStream_t st, View<R> out, View<const R> Q_basis, View<const R> Q_coeff, View<const R> Rm);
 
-// rhs[i, :] <- rhs[perm[i], :] for every scalar kind (perm: HOST int64 of rhs.nrows entries; the row gather of the LU /
-// QR reconstructions); a column permutation is this on the transposed view
-template <class R, bool CX>
-void permute_rows_t(cudaStream_t st, View<R> rhs, const long long* perm);
 // out[i, j] <- src[p[i], q[j]] for every scalar kind (p, q: HOST int64 of out.nrows / out.ncols entries; out and src must not
 // overlap); the permuted 2-D gather of the full-pivoting LU reconstruct / inverse
 template <class R, bool CX>
 void gather_2d_t(cudaStream_t st, View<R> out, View<const R> src, const long long* p, const long long* q);
-// cplx.cu: T(strict upper) <- V^H V for complex reflectors (upgrade_householder_factor with prev_block_size 1; views in COMPLEX
-// element units on an R* base), the twin of householder_build_t
-template <class R>
-void householder_build_t_cx(cudaStream_t st, View<const R> V, View<R> Tf);
 
 // dst(triangle) <- src(triangle)^-1 (triangular_inverse.rs), every scalar kind; only the triangle is written (not the diagonal if unit)
 template <class R, bool CX>

@@ -293,7 +293,7 @@ void libfaer_v0_23_inverse_unit_triangular_upper_in_place_c32(struct FaerV0_24_M
  * semantics: cholesky/llt/reconstruct.rs:12-33 and inverse.rs:10-39 (only the LOWER triangle of the output is written),
  * lu/partial_pivoting/reconstruct.rs and inverse.rs, qr/no_pivoting/reconstruct.rs:13-39 and inverse.rs. L / U may be the packed
  * LU matrix or the split factors (the excluded parts are never read). The LU and QR inverses are the solves applied to the
- * identity (csrc/reconstruct.cu). */
+ * identity (csrc/reconstruct_types.cu). */
 struct FaerV0_24_Layout libfaer_v0_23_llt_reconstruct_scratch_f64(size_t dim, struct FaerV0_24_Par par);
 void libfaer_v0_23_llt_reconstruct_f64(struct FaerV0_24_MatMut A, struct FaerV0_24_MatRef L, struct FaerV0_24_Par par, struct FaerV0_24_MemAlloc mem);
 struct FaerV0_24_Layout libfaer_v0_23_llt_inverse_scratch_f64(size_t dim, struct FaerV0_24_Par par);

@@ -187,7 +187,7 @@ def test_self_adjoint_evd_driver(drv, dtype):
 
 
 # ---- reconstruct_types.cu --------------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("dtype", [np.float32, np.complex128, np.complex64])
+@pytest.mark.parametrize("dtype", [np.float64, np.float32, np.complex128, np.complex64])
 def test_reconstruct_types_drivers(drv, oracle, dtype):
     rng = np.random.default_rng(1702)
     u = float(np.finfo(rdt(dtype)).eps)

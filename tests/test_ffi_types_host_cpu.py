@@ -1,4 +1,4 @@
-"""The C-ABI entry points added for f32 / c64 / c32 (`*_reconstruct` / `*_inverse`, LDLT, complex `svd` / `self_adjoint_evd`) run on
+"""The C-ABI entry points of csrc/ffi_types.cu (`*_reconstruct` / `*_inverse`, LDLT, complex `svd` / `self_adjoint_evd`) run on
 the CPU through the real Python binding: tools/emul/ffi_types_host.cpp builds csrc/ffi_types.cu + runtime.cu (entry lock, workspace
 pool, StagedMat staging) + the three flat-map drivers, as they are, against a host stand-in of <cuda_runtime.h>; `capi.load()` is
 pointed at that library and THE GPU TESTS' OWN FUNCTIONS are executed — same arrays, same views, same assertions as on the GPU.
@@ -68,21 +68,21 @@ def hostlib(tmp_path_factory, fb, oracle):
     for suf in ("f64", "f32", "c64", "c32"):
         for name in ("ldlt_reconstruct", "ldlt_inverse"):
             g(f"{name}_{suf}").argtypes = [MatMut, MatRef, VecMut, P, MemAlloc]; g(f"{name}_{suf}").restype = None
-        if suf == "f64":
-            continue
         for name in ("llt_reconstruct", "llt_inverse"):
             g(f"{name}_{suf}").argtypes = [MatMut, MatRef, P, MemAlloc]; g(f"{name}_{suf}").restype = None
         for it in ("u32", "u64"):
             for name in ("partial_piv_lu_reconstruct", "partial_piv_lu_inverse"):
                 g(f"{name}_{it}_{suf}").argtypes = [MatMut, MatRef, MatRef, SliceMut, SliceMut, P, MemAlloc]; g(f"{name}_{it}_{suf}").restype = None
-        if suf != "f32":
-            g(f"qr_reconstruct_{suf}").argtypes = [MatMut, MatRef, MatRef, MatRef, P, MemAlloc]; g(f"qr_reconstruct_{suf}").restype = None
+        for name in ("qr_reconstruct", "qr_inverse"):
+            g(f"{name}_{suf}").argtypes = [MatMut, MatRef, MatRef, MatRef, P, MemAlloc]; g(f"{name}_{suf}").restype = None
+        if suf in ("c64", "c32"):
             g(f"SvdParams_{suf}").argtypes = []; g(f"SvdParams_{suf}").restype = capi.SvdParams
             g(f"svd_{suf}").argtypes = [MatRef, MatMut, VecMut, MatMut, P, MemAlloc, capi.SvdParams]; g(f"svd_{suf}").restype = capi.SvdStatus
             g(f"SelfAdjointEvdParams_{suf}").argtypes = []; g(f"SelfAdjointEvdParams_{suf}").restype = capi.SelfAdjointEvdParams
             g(f"self_adjoint_evd_{suf}").argtypes = [MatRef, MatMut, VecMut, P, MemAlloc, capi.SelfAdjointEvdParams]
             g(f"self_adjoint_evd_{suf}").restype = capi.EvdStatus
-        g(f"qr_inverse_{suf}").argtypes = [MatMut, MatRef, MatRef, MatRef, P, MemAlloc]; g(f"qr_inverse_{suf}").restype = None
+        if suf == "f64":
+            continue                                                      # the f64 LDLT factorization is ldlt_f64.cu, not in this library
         g(f"LdltParams_{suf}").argtypes = []; g(f"LdltParams_{suf}").restype = capi.LdltParams
         g(f"ldlt_factor_in_place_{suf}").argtypes = [MatMut, capi.LdltRegularization, P, MemAlloc, capi.LdltParams]
         g(f"ldlt_factor_in_place_{suf}").restype = capi.LdltStatus
@@ -131,21 +131,11 @@ def host_fb(fb, oracle, hostlib, monkeypatch):
             raise la.LdltError(fail)
         return la.LdltInfo(count)
 
-    real_qr_reconstruct = la.qr_reconstruct
-
-    def qr_reconstruct(out, Q_basis, Q_coeff, R, par=None):
-        if out.dtype != np.float32:
-            return real_qr_reconstruct(out, Q_basis, Q_coeff, R, par)     # the host library's own entry point
-        size = min(out.shape)                                             # qr_reconstruct_f32 lives in ffi.cu (validated on hardware)
-        out[...] = 0
-        out[:size, :] = np.triu(R[:size, :])
-        oracle.apply_q_sequence(np.asfortranarray(Q_basis), Q_coeff, out, conj_lhs=False)
-
     def matmul(dst, accum, lhs, rhs, alpha, par=None):
         oracle.matmul(dst, accum == la.Accum.Add, np.asarray(lhs), np.asarray(rhs), alpha)
 
     for name, f in (("cholesky_in_place", cholesky_in_place), ("lu_in_place", lu_in_place), ("qr_in_place", qr_in_place),
-                    ("ldlt_in_place", ldlt_in_place), ("matmul", matmul), ("qr_reconstruct", qr_reconstruct),
+                    ("ldlt_in_place", ldlt_in_place), ("matmul", matmul),
                     ("qr_recommended_block_size", oracle.qr_recommended_block_size)):
         monkeypatch.setattr(la, name, f)
     return fb

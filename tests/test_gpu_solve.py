@@ -34,7 +34,7 @@ def test_lu_solve(fb, oracle, cuda_dev, idx):
     import torch
     la = fb.linalg
     rng = np.random.default_rng(32)
-    for n, k in [(1, 1), (50, 3), (200, 7), (400, 130), (1000, 16)]:
+    for n, k in [(1, 1), (50, 3), (200, 7), (400, 130), (1000, 16), (3, 65537)]:
         A = np.asfortranarray(rng.standard_normal((n, n)))
         B = np.asfortranarray(rng.standard_normal((n, k)))
         LU = A.copy(order="F"); p = np.zeros(n, idx); pi = np.zeros(n, idx)

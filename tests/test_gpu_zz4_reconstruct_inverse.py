@@ -1,4 +1,4 @@
-"""`*_reconstruct` / `*_inverse` on the factors through the C ABI (csrc/reconstruct.cu; compositions of validated kernels).
+"""`*_reconstruct` / `*_inverse` on the factors through the C ABI (csrc/reconstruct_types.cu; compositions of validated kernels).
 Reference tests restated for f64:
 llt/reconstruct.rs and inverse.rs tests (n = 50, eps * n), lu/partial_pivoting/reconstruct.rs and inverse.rs tests,
 qr/no_pivoting/reconstruct.rs tests ((100, 50) and (50, 100)) and inverse.rs tests."""

@@ -1,16 +1,16 @@
-"""`*_reconstruct` / `*_inverse` on the factors for f32 / c64 / c32 through the C ABI (csrc/reconstruct_types.cu: the f64
-compositions of reconstruct.cu over the products, solves and Householder sequences of each scalar kind).
+"""`*_reconstruct` / `*_inverse` on the factors for f64 / f32 / c64 / c32 through the C ABI (csrc/reconstruct_types.cu: one
+composition over the products, solves and Householder sequences of each scalar kind).
 The reference's own tests restated per dtype (they draw complex matrices):
   cholesky/llt/reconstruct.rs + inverse.rs tests (n = 50), lu/partial_pivoting/reconstruct.rs tests ((100, 50), (50, 100),
   (50, 50)) + inverse.rs tests (n = 50), qr/no_pivoting/reconstruct.rs tests ((100, 50), (50, 100)) + inverse.rs tests (n = 50),
-plus sizes that cross the block boundaries of the kernels underneath. The f64 entry points stay covered by
+plus sizes that cross the block boundaries of the kernels underneath. The f64 entry points are also covered by
 test_gpu_zz4_reconstruct_inverse.py; here the f64 results also serve as the cross-check of the f32 ones."""
 import numpy as np
 import pytest
 
 pytestmark = pytest.mark.gpu
 
-DTYPES = [np.float32, np.complex128, np.complex64]
+DTYPES = [np.float64, np.float32, np.complex128, np.complex64]
 
 
 def _rand(rng, shape, dtype):

@@ -1,4 +1,4 @@
-"""The compositions of csrc/reconstruct_types.cu (`*_reconstruct` / `*_inverse` on the factors for f32 / c64 / c32), restated call
+"""The compositions of csrc/reconstruct_types.cu (`*_reconstruct` / `*_inverse` on the factors), restated call
 for call on the oracle's building blocks with the SAME structure codes and conjugation flags the CUDA file passes to the GPU's
 products, solves and Householder sequences (which are tested against these very oracle functions on hardware). Pins the one
 non-mechanical part of that file — which operand is conjugated, which sequence is applied — on the CPU:
@@ -72,7 +72,7 @@ def qr_reconstruct(orc, out, Qb, Qc, R):
 def qr_inverse(orc, out, Qb, Qc, R):
     n = out.shape[0]
     out[...] = np.eye(n, dtype=out.dtype)
-    orc.apply_q_transpose_sequence(Qb, Qc, out, conj_lhs=True)   # rt_hh_seq(adjoint = true): conj = transpose = true
+    orc.apply_q_transpose_sequence(Qb, Qc, out, conj_lhs=True)   # householder_sequence_t with conj = transpose = true
     orc.solve_triangular(R, out, lower=False, unit=False, conj=False)
 
 

@@ -106,6 +106,7 @@ int drv_evd(int is_double, MockMat A, MockMat U, void* S, long long sstride) {
 void drv_recon(int kind, int which, MockMat out, MockMat a, MockMat b, MockMat c, const long long* perm) {
   switch (kind) {
     case 0: recon<float, false>(which, out, a, b, c, perm); break;
+    case 1: recon<double, false>(which, out, a, b, c, perm); break;
     case 2: recon<float, true>(which, out, a, b, c, perm); break;
     case 3: recon<double, true>(which, out, a, b, c, perm); break;
   }
